@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- the hot path of MMRec on B200, measured per BASELINE.json.
+"""bench.py -- the hot path of MMRec on H100, measured per BASELINE.json.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --steps K --warmup W    # the reference's CPU algorithm (oracle port)
+    python bench.py --steps K --warmup W --dump-outputs DIR  # + the last timed step's outputs as DIR/<name>.npy
 
 Workload (N=1): BASELINE.json configs[1] -- FREEDOM on the synthetic baby-shaped graph (20k users, 7k items,
 160k train edges, d=64, 3 UI layers + 1 item-graph layer), then full-catalog scoring + mask + top-50 for every
@@ -41,16 +42,8 @@ def peaks():
     if os.path.isfile(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "src": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "src": "fallback (B200_PROFILING.md)"}
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed ncu --set full capture
-    (profiles/traffic.json, written by tools/summarize_ncu.py); None when no capture is recorded."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))[kernel]["dram_bytes_per_launch"]
-    except Exception:
-        return None
+    # NVIDIA's data sheet for the H100 SXM (700 W): HBM3 bandwidth, dense BF16 / FP16 tensor rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "src": "fallback (H100 SXM data sheet)"}
 
 
 class ClockSampler:
@@ -235,6 +228,23 @@ def forward_eval(model):
     return model.forward()
 
 
+def dump_outputs(out_dir, outs):
+    """The arrays the timed sections hand their caller, from the last replay of each section's CUDA graph: the
+    propagated user / item embeddings ([A]), both modality projections ([B]) and the top-k index matrix of all users
+    ([C]; int64 indices written as float64, exact below 2^53)."""
+    os.makedirs(out_dir, exist_ok=True)
+    named = {}
+    if "a" in outs:
+        named["prop_user_emb"], named["prop_item_emb"] = outs["a"]
+    if "b" in outs:
+        named["proj_image"], named["proj_text"] = outs["b"]
+    if "c" in outs:
+        named["topk_idx"] = outs["c"]
+    for name, t in named.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64 if a.dtype.kind in "iu" or a.dtype == np.float64 else np.float32))
+
+
 def torch_gpu_comparator(model, u_users, batches_dev, flush, reps=5):
     """The reference's own formulation on the same GPU with stock PyTorch kernels -- un-coalesced COO adjacency through
     `torch.sparse.mm` per layer + `stack().mean()` (`src/models/freedom.py:164-178`), `matmul` + in-place mask +
@@ -344,7 +354,7 @@ def bench_model(wl, model_name, dev, args, flush, sampler=None, full=True):
         for step in range(warm + steps):
             if step == 0 and sampler is not None:
                 sampler.start()
-            flush.zero_()                                            # evict L2 (126 MB) between steps
+            flush.zero_()                                            # evict L2 (50 MB) between steps
             marks = []
             for name, _ in secs:
                 e0, e1 = ev(), ev()
@@ -355,6 +365,8 @@ def bench_model(wl, model_name, dev, args, flush, sampler=None, full=True):
                 for name, e0, e1 in marks:
                     times[name] += e0.elapsed_time(e1)
     ms = {k: v / steps for k, v in times.items()}
+    if full and getattr(args, "dump_outputs", None):
+        dump_outputs(args.dump_outputs, {name: graphs[name][1] for name, _ in secs})
     launches = sum(n_launch[k] for k in n_launch if k != "c4096") * steps      # (the 4096-batch variant is an extra, not part of the step)
 
     # ---- e2e through the same model calls, HOST buffers (pinned), copies inside the timed region.  [A]: the embedding
@@ -500,9 +512,9 @@ def run_ours(args):
                   "score_path": os.environ.get("MMREC_SCORE_PATH", "auto"), "torch_gpu_comparator": r.get("torch_gpu_comparator")},
         "roofline": {"kernel": "spmm_vec_kernel<64,16> (the SpMMs of one forward: 3 x A_hat + mm_adj)", "bound": "hbm",
                      "achieved": spmm_bytes / (msA * 1e-3) / 1e9, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                     "frac": spmm_bytes / (msA * 1e-3) / 1e9 / pk["hbm_gbs"], "traffic": ncu_traffic("spmm_vec_kernel"), "peak_src": pk["src"],
+                     "frac": spmm_bytes / (msA * 1e-3) / 1e9 / pk["hbm_gbs"], "peak_src": pk["src"],
                      "algorithmic_bytes_per_launch_ui": r["ui_bytes"]},
-        "roofline_scoring": {"kernel": "cf_pass_kernel<1|2> (tcgen05 kind::f16 on fp16-rounded operands, two passes) + cf_thr / cf_final "
+        "roofline_scoring": {"kernel": "cf_pass_kernel<1|2> (wgmma f16 on fp16-rounded operands, two passes) + cf_thr / cf_final "
                                        "(+ operand packing, mask CSR)",
                              "bound": "tensor", "achieved": r["score_flops"] / (msC * 1e-3) / 1e12, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
                              "frac": r["score_flops"] / (msC * 1e-3) / 1e12 / pk["bf16_tflops"],
@@ -657,6 +669,8 @@ def main():
     ap.add_argument("--sharded", action="store_true", help="run the item-sharded driver also at --gpus 1 (weak-scaling baseline)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-other-configs", action="store_true", help="skip the BM3/sports and MGCN/clothing lines in extra")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

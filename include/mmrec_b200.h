@@ -1,4 +1,4 @@
-/* mmrec_b200 -- C ABI of the B200-native hot path of MMRec.
+/* mmrec_b200 -- C ABI of the H100-native hot path of MMRec.
  *
  * The reference (enoche/MMRec, /root/reference) is pure Python on PyTorch; it has no FFI of
  * its own.  Its "plugin boundary" is the model class contract of
@@ -31,7 +31,7 @@ extern "C" {
 #define MMREC_EINVAL (-1)      /* bad argument (null pointer, negative size, unsupported d or k) */
 #define MMREC_EWORKSPACE (-2)  /* ws_bytes smaller than *_workspace_bytes() */
 #define MMREC_ECUDA (-3)       /* a CUDA runtime call failed; see mmrec_last_error() */
-#define MMREC_EUNSUPPORTED (-4)/* device is not sm_100 (the library carries sm_100a code only) */
+#define MMREC_EUNSUPPORTED (-4)/* device is not sm_90 (the library carries sm_90a code only) */
 
 #define MMREC_ABI_VERSION 3
 
@@ -147,7 +147,7 @@ int mmrec_spmm_chain_f32(int d, int n_steps, const mmrec_spmm_step* steps, void*
  * bm3.py:102-104, mgcn.py:148-150) and `F.normalize(MLP(features))` (mmgcn.py:165-168).
  *   Y[n,:] = table[idx ? idx[n] : n, :] @ W^T + bias      table [n_table, F], W [d, F], bias [d]|NULL
  *   l2_normalize: Y[n,:] /= max(||Y[n,:]||_2, 1e-12)
- * Two arithmetic paths: tcgen05 3xTF32 with the table split in-kernel (default when ws is given and d <= 256;
+ * Two arithmetic paths: wgmma 3xTF32 with the table split in-kernel (default when ws is given and d <= 256;
  * ws from mmrec_project_workspace_bytes holds the re-tiled weights and the K-split partials) and exact fp32 on CUDA
  * cores (ws == NULL, or mmrec_project_set_path(0) / env MMREC_PROJECT_PATH=simt).
  * ------------------------------------------------------------------------------------------- */
@@ -157,8 +157,8 @@ int mmrec_project_f32(int64_t n_out, const int64_t* idx, const float* table, int
                       const float* W, const float* bias, int d, int l2_normalize,
                       float* Y, int64_t ldy, void* ws, size_t ws_bytes, void* stream);
 
-/* measurement aid (tools/probe_mma.py): cycles of `iters` back-to-back tcgen05.mma (cta_group::1, operands in shared memory,
- * K-major no swizzle, M = 128, K = 32 bytes) per CTA, one CTA per SM; kind 0 = tf32, 1 = bf16 */
+/* measurement aid (tools/probe_mma.py): cycles of `iters` back-to-back wgmma (one warpgroup, operands in shared memory,
+ * K-major no swizzle, M = 64, K = 32 bytes) per CTA, one CTA per SM; kind 0 = tf32, 1 = bf16 */
 int mmrec_debug_mma_rate(int kind, int N, int iters, int distinct, long long* cycles_per_cta, void* stream);
 
 /* measurement aid (tools/probe_stream.py): stream a [n_rows, F] fp32 table the way K2 does -- every CTA visits R rows
@@ -196,7 +196,7 @@ int mmrec_debug_stream_probe(const float* table, int64_t n_rows, int64_t F, int 
  * ------------------------------------------------------------------------------------------- */
 /* path of mmrec_score_f32 / mmrec_score_topk_f32 (env MMREC_SCORE_PATH = simt | tc | auto | fused sets the start value):
  *   0 simt   exact fp32 on CUDA cores
- *   1 tc     tcgen05 3xTF32 GEMM into an L2-resident score block, then mask + radix-select top-k kernels
+ *   1 tc     wgmma 3xTF32 GEMM into an L2-resident score block, then mask + radix-select top-k kernels
  *   2 auto   (default) fused wherever its shape rules allow (k <= 256, d <= 128, at least 2k item groups of 16..128
  *            items), else tc
  *   3 fused  certified-filter path, no score matrix */

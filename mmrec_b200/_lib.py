@@ -115,8 +115,8 @@ def check(rc: int, what: str):
 
 
 def require_device():
-    """Fail loudly unless a B200-class (sm_100) device is current."""
+    """Fail loudly unless an H100-class (sm_90) device is current."""
     import torch
     if not torch.cuda.is_available():
-        raise MMRecError("mmrec_b200 needs a CUDA device (sm_100a); there is no CPU path")
+        raise MMRecError("mmrec_b200 needs a CUDA device (sm_90a); there is no CPU path")
     check(load().mmrec_device_check(), "mmrec_device_check")

@@ -1,6 +1,6 @@
 """Model-side boundary of the hot path: the class contract the reference's trainer drives.
 
-Mirrors `/root/reference/src/common/abstract_recommender.py:10-103` (same method names, attributes and config
+Mirrors `src/common/abstract_recommender.py:10-103` (same method names, attributes and config
 keys) so that the model classes in `mmrec_b200.models` are drop-ins under the reference's `src/models`
 (see INTEGRATION.md).  Extra, optional entry point used by this repo's trainer:
 `full_sort_topk(interaction, k)` -- the fused scoring + mask + top-k fast path.

@@ -1,4 +1,4 @@
-"""Loss modules with the reference's semantics (`/root/reference/src/common/loss.py:9-62`); plain torch, not on
+"""Loss modules with the reference's semantics (`src/common/loss.py:9-62`); plain torch, not on
 the kernel path (SURVEY.md 2.1 #9)."""
 import torch
 import torch.nn as nn

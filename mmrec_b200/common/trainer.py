@@ -1,4 +1,4 @@
-"""Training / evaluation driver with the reference's control flow (`/root/reference/src/common/trainer.py`):
+"""Training / evaluation driver with the reference's control flow (`src/common/trainer.py`):
 same optimiser construction (`:111-128`), epoch loop with NaN abort and early stopping (`:223-289`) and
 evaluation protocol (`:292-311`).  Differences, all on the hot path:
 

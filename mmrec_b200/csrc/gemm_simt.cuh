@@ -2,7 +2,7 @@
 // This is the bit-faithful fp32 path (one fmaf chain per output, k ascending) used by
 //   * mmrec_project_f32  (M = rows to project, N = d, K = F)       -- src/models/freedom.py:205-209
 //   * mmrec_score_f32    (M = users, N = items, K = d)             -- src/models/freedom.py:219
-// and the yardstick the tcgen05 kernels are validated against on the device.
+// and the yardstick the tensor-core kernels are validated against on the device.
 #pragma once
 #include "common.cuh"
 

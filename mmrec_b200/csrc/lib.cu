@@ -18,10 +18,10 @@ void set_error(const char* fmt, ...) {
 int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (!cached[dev]) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev] = n;
     }
     return cached[dev];
@@ -44,8 +44,8 @@ extern "C" int mmrec_device_check(void) {
         mmrec::set_error("device_check: no CUDA device: %s", cudaGetErrorString(cudaGetLastError()));
         return MMREC_ECUDA;
     }
-    if (major != 10) {
-        mmrec::set_error("device_check: compute capability %d.x, this library carries sm_100a code only", major);
+    if (major != 9) {
+        mmrec::set_error("device_check: compute capability %d.x, this library carries sm_90a code only", major);
         return MMREC_EUNSUPPORTED;
     }
     return MMREC_OK;

@@ -1,5 +1,5 @@
 // K2: fused gather -> linear(+bias) -> optional L2 normalise (exact-fp32 CUDA-core path).
-// The tensor-core (tcgen05, 3xTF32) variant lives in project_tc.cu; this file is the bit-faithful
+// The tensor-core (wgmma, 3xTF32) variant lives in project_tc.cu; this file is the bit-faithful
 // fp32 path and the fallback for widths the tensor-core tiles do not cover.
 #include "gemm_simt.cuh"
 
@@ -14,7 +14,7 @@ int project_tc(int64_t n_out, const int64_t* idx, const float* table, int64_t F,
                int l2_normalize, float* Y, int64_t ldy, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t project_tc_workspace_bytes(int64_t n_out, int64_t F, int d);
 
-static int g_project_path = -1;   // 0 = exact fp32 CUDA cores, 1 = tcgen05 3xTF32 (default)
+static int g_project_path = -1;   // 0 = exact fp32 CUDA cores, 1 = wgmma 3xTF32 (default)
 static int project_path() {
     if (g_project_path < 0) {
         const char* e = getenv("MMREC_PROJECT_PATH");

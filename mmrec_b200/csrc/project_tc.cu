@@ -1,16 +1,19 @@
-// K2 on the tensor cores: Y = gather(table, idx) @ W^T (+ bias, optional row L2-norm) with tcgen05.mma kind::tf32 and
-// the 3xTF32 split (fp32-level accuracy; the bar for projections is 1e-4 relative, single-pass TF32 misses it).
+// K2 on the tensor cores: Y = gather(table, idx) @ W^T (+ bias, optional row L2-norm) with wgmma (tf32) and the 3xTF32
+// split (fp32-level accuracy; the bar for projections is 1e-4 relative, single-pass TF32 misses it).
 //
 // The feature table is the big operand (115 MB at 7k x 4096) and is read from HBM exactly once, as fp32, so its hi/lo
 // split happens IN the kernel:
-//   converter warps (8)  coalesced 16-byte loads of the gathered rows (two register rings of 4 K chunks: 64 KB per SM in
-//                        flight while 64 KB are converted; 512 contiguous bytes per row visit), split each value into
-//                        tf32 hi (mantissa truncated to 10 bits) + lo (the exact remainder, which the tensor core truncates), store both into shared memory directly in the UMMA canonical
-//                        K-major layout (8 x 16 B core matrices; K stride padded to 2064 B so the stores are
-//                        conflict-free), fence.proxy.async, arrive on the stage's mbarrier;
+//   converter warps (8)  two warpgroups.  Coalesced 16-byte loads of the gathered rows (two register rings of PJ_DEPTH
+//                        K chunks: one in flight while the other is converted; 384 contiguous bytes per row visit at
+//                        N = 64), split each value into tf32 hi (mantissa truncated to 10 bits) + lo (the exact
+//                        remainder, which the tensor core truncates), store both into shared memory directly in the
+//                        canonical K-major layout of wgmma (8 x 16 B core matrices; K stride padded to 2064 B so the
+//                        stores are conflict-free), fence.proxy.async, arrive on the stage's mbarrier.  Once the whole
+//                        stage is in (both warpgroups + the weights), each warpgroup issues 12 x wgmma M64 N{64,128,256}
+//                        K8 per 32-wide K chunk (hi.hi + lo.hi + hi.lo) for its 64 rows of the tile into registers,
+//                        keeps one chunk's group in flight and hands the stage before it back;
 //   producer warp        cp.async.bulk of the pre-split, pre-tiled weight slab (hi and lo) of the same K chunk;
-//   MMA warp             12 x tcgen05.mma M128 N{64,128,256} K8 per 32-wide K chunk: hi.hi + lo.hi + hi.lo;
-//   epilogue             four of the converter warps read the accumulator (tcgen05.ld) and write one fp32 partial per K split.
+//   epilogue             the accumulator registers are written as one fp32 partial per K split.
 // Grid = row tiles x K splits <= SM count (one wave); project_reduce_kernel adds the K splits, the bias and applies
 // the row normalisation.  Per launch the kernel moves 4 n F (+ weights) bytes for 2 n F d useful flops -> HBM-bound.
 #include "tc_common.cuh"
@@ -23,9 +26,12 @@ constexpr int PJ_M = 128;                 // rows per CTA tile
 constexpr int PJ_KC = 32;                 // k per stage
 constexpr int PJ_LBO_A = 2064;            // 16 row groups x 128 B + 16 B pad: K-adjacent core matrices land on different banks
 constexpr int PJ_A_BYTES = (PJ_KC / 4) * PJ_LBO_A;            // one of hi / lo for one stage = 16512 B
-constexpr int PJ_CONV = 256;              // converter threads (8 warps); the first 4 of them also run the epilogue
-constexpr int PJ_DEPTH = 4;               // chunks of table reads in flight per converter thread (64 KB per SM)
-constexpr int PJ_THREADS = 64 + PJ_CONV;  // warp 0 weight producer, warp 1 MMA, warps 2..9 converters
+constexpr int PJ_CONV = 256;              // converter threads = the two MMA warpgroups
+constexpr int PJ_THREADS = PJ_CONV + 32;  // warps 0..7 converters / MMA, warp 8 weight producer
+// chunks of table reads in flight per converter thread (16 KB per SM and chunk).  A block that issues wgmma is sized
+// in whole warpgroups (288 -> 384 threads: at most 168 registers per thread), so the ring shrinks as N's accumulators
+// grow (N = 256 still spills a few)
+template <int N> constexpr int pj_depth() { return N == 64 ? 3 : (N == 128 ? 2 : 1); }
 
 struct ProjParams {
     const float* table; int64_t F; const int64_t* idx; int64_t n_out;
@@ -36,7 +42,7 @@ struct ProjParams {
 };
 
 struct PjSmem {
-    uint32_t a0, b0, bars, tmem_ptr, total, stage_bytes, b_bytes;
+    uint32_t a0, b0, bars, total, stage_bytes, b_bytes;
 };
 __host__ __device__ inline PjSmem pj_smem(int N, int stages) {
     PjSmem L;
@@ -45,30 +51,24 @@ __host__ __device__ inline PjSmem pj_smem(int N, int stages) {
     L.a0 = 0;
     L.b0 = 2 * PJ_A_BYTES;                                     // inside a stage: A_hi | A_lo | B_hi | B_lo
     L.bars = stages * L.stage_bytes;
-    L.tmem_ptr = L.bars + 32 * 8;
-    L.total = L.tmem_ptr + 16;
+    L.total = L.bars + 32 * 8;
     return L;
 }
-// barriers: a_full[s] = 0..7 (PJ_CONV arrivals) | b_full[s] = 8..15 (tx) | empty[s] = 16..23 (1, tcgen05.commit) | acc_full = 24
+// barriers: a_full[s] = 0..7 (PJ_CONV arrivals) | b_full[s] = 8..15 (tx) | empty[s] = 16..23 (one arrival per converter warp)
 
-template <bool FAST>
+template <int N, bool FAST>
 __global__ void __launch_bounds__(PJ_THREADS, 1) project_tc_kernel(const ProjParams p) {
+    constexpr int PJ_DEPTH = pj_depth<N>();
     extern __shared__ __align__(1024) uint8_t smem[];
-    const PjSmem L = pj_smem(p.N, p.stages);
+    const PjSmem L = pj_smem(N, p.stages);
     const uint32_t sbase = smem_u32(smem);
     const uint32_t bar = sbase + L.bars;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < 8; ++s) { mbar_init(bar + s * 8, PJ_CONV); mbar_init(bar + (8 + s) * 8, 1); mbar_init(bar + (16 + s) * 8, 1); }
-        mbar_init(bar + 24 * 8, 1);
+        for (int s = 0; s < 8; ++s) { mbar_init(bar + s * 8, PJ_CONV); mbar_init(bar + (8 + s) * 8, 1); mbar_init(bar + (16 + s) * 8, PJ_CONV / 32); }
         mbar_fence_init();
     }
-    const uint32_t tmem_cols = p.N < 32 ? 32 : p.N;
-    if (warp == 1) { tmem_alloc(sbase + L.tmem_ptr, tmem_cols); tmem_relinquish(); }
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + L.tmem_ptr);
 
     const int tile = blockIdx.x / p.n_splits, sp = blockIdx.x % p.n_splits;
     const int c0 = sp * p.chunks_per_split;
@@ -76,11 +76,11 @@ __global__ void __launch_bounds__(PJ_THREADS, 1) project_tc_kernel(const ProjPar
     const int n_my = c1 - c0;
     // K rotation: CTA `tile` starts its K loop at a different chunk.  With a power-of-two row pitch (F = 4096: 16 KB) all
     // CTAs would otherwise read the same few-hundred-byte window of every row at the same time -- the same address bits,
-    // hence the same few HBM channels (measured: 20 % of peak, 4.5 us load latency).  Spreading the windows over the
-    // row restores the channel interleave; the accumulation order differs per row tile but not run to run.
+    // hence the same few HBM channels.  Spreading the windows over the row restores the channel interleave; the
+    // accumulation order differs per row tile but not run to run.
     const int rot = n_my > 0 ? ((int)(((int64_t)tile * n_my) / p.n_tiles) / PJ_DEPTH * PJ_DEPTH) % n_my : 0;
 
-    if (warp == 0) {
+    if (warp == PJ_CONV / 32) {
         if (lane == 0) {
             int s = 0;
             uint32_t par = 1;
@@ -93,143 +93,134 @@ __global__ void __launch_bounds__(PJ_THREADS, 1) project_tc_kernel(const ProjPar
                 if (++s == p.stages) { s = 0; par ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = idesc_tf32(PJ_M, p.N);
-            const uint32_t LBO_B = (uint32_t)(p.N / 8) * 128;
-            uint32_t acc = 0;
-            int s = 0;
-            uint32_t par = 0;
-            // one thread's instruction stream feeds the tensor pipe: the four descriptors are built once and only their
-            // address field (16-byte units, low word) moves -- rebuilding them per instruction costs ~200 cycles per MMA
-            // against ~90 for the MMA itself (tools/probe_mma.py)
-            const uint64_t a_hi0 = smem_desc(sbase + L.a0, PJ_LBO_A, 128), a_lo0 = smem_desc(sbase + L.a0 + PJ_A_BYTES, PJ_LBO_A, 128);
-            const uint64_t b_hi0 = smem_desc(sbase + L.b0, LBO_B, 128), b_lo0 = smem_desc(sbase + L.b0 + L.b_bytes, LBO_B, 128);
-            const uint64_t ka = (2 * PJ_LBO_A) >> 4, kb = (2 * LBO_B) >> 4, st_step = L.stage_bytes >> 4;
-            uint64_t st = 0;
-            for (int c = 0; c < n_my; ++c) {
-                mbar_wait(bar + s * 8, par);
-                mbar_wait(bar + (8 + s) * 8, par);
-                fence_after_sync();
-                uint64_t a_hi = a_hi0 + st, a_lo = a_lo0 + st, b_hi = b_hi0 + st, b_lo = b_lo0 + st;
+        return;
+    }
+    // ---------------- converters: thread t owns kblk t % 8 of rows t / 8 + 32 i, i = 0..3; PJ_DEPTH chunks of its
+    // 16-byte reads are in flight at any time (registers are the staging buffer)
+    const int t = threadIdx.x;
+    const int g = t >> 7;                                             // warpgroup: MMA rows [64 g, 64 g + 64) of the tile
+    const int kb = t & 7;
+    const float* rowp[4];
 #pragma unroll
-                for (int j = 0; j < PJ_KC / 8; ++j) {
-                    mma_tf32(tmem_base, a_hi, b_hi, idesc, acc);
-                    acc = 1;
-                    mma_tf32(tmem_base, a_lo, b_hi, idesc, 1);
-                    mma_tf32(tmem_base, a_hi, b_lo, idesc, 1);
-                    a_hi += ka; a_lo += ka; b_hi += kb; b_lo += kb;
-                }
-                mma_commit(bar + (16 + s) * 8);
-                st += st_step;
-                if (++s == p.stages) { s = 0; par ^= 1; st = 0; }
-            }
-            mma_commit(bar + 24 * 8);
+    for (int i = 0; i < 4; ++i) {
+        const int64_t r = (int64_t)tile * PJ_M + (t >> 3) + 32 * i;
+        rowp[i] = r < p.n_out ? p.table + (p.idx ? p.idx[r] : r) * p.F : nullptr;
+    }
+    // FAST (16-byte aligned table, F a multiple of 32: every BASELINE shape): the loop is bound by the instruction stream
+    // of the 8 converter warps, so the chunk rotation is a running counter instead of a modulo, and a load is one
+    // predicated 16-byte request per row.
+    int ld_c = rot;                                               // chunk (inside this split) the next load reads
+    const float* kp[4];                                           // FAST: row pointers advanced to this thread's k block
+#pragma unroll
+    for (int i = 0; i < 4; ++i) kp[i] = rowp[i] ? rowp[i] + (int64_t)c0 * PJ_KC + kb * 4 : nullptr;
+    auto load_chunk = [&](int c, float4 (&x)[4]) {
+        if (FAST) {
+            const bool on = c < n_my;                             // (warp-uniform)
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                x[i] = (on && kp[i]) ? __ldg(reinterpret_cast<const float4*>(kp[i] + ld_c * PJ_KC)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            if (on && ++ld_c == n_my) ld_c = 0;
+            return;
         }
-    } else {
-        // ---------------- converters: thread t owns kblk t % 8 of rows t / 8 + 32 i, i = 0..3; PJ_DEPTH chunks of its
-        // 16-byte reads are in flight at any time (registers are the staging buffer: 256 thr x 4 x 4 x 16 B = 64 KB per SM)
-        const int t = threadIdx.x - 64;
-        const int kb = t & 7;
-        const float* rowp[4];
+        const int64_t k = (int64_t)(c0 + (c + rot) % n_my) * PJ_KC + kb * 4;    // (c >= n_my: not loaded, see below)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const int64_t r = (int64_t)tile * PJ_M + (t >> 3) + 32 * i;
-            rowp[i] = r < p.n_out ? p.table + (p.idx ? p.idx[r] : r) * p.F : nullptr;
-        }
-        // FAST (16-byte aligned table, F a multiple of 32: every BASELINE shape): the loop is bound by the instruction stream
-        // of the 8 converter warps (measured: 236 instructions per chunk and warp at one issue per ~8.5 cycles), so the chunk
-        // rotation is a running counter instead of a modulo, and a load is one predicated 16-byte request per row.
-        int ld_c = rot;                                               // chunk (inside this split) the next load reads
-        const float* kp[4];                                           // FAST: row pointers advanced to this thread's k block
-#pragma unroll
-        for (int i = 0; i < 4; ++i) kp[i] = rowp[i] ? rowp[i] + (int64_t)c0 * PJ_KC + kb * 4 : nullptr;
-        auto load_chunk = [&](int c, float4 (&x)[4]) {
-            if (FAST) {
-                const bool on = c < n_my;                             // (warp-uniform)
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-                    x[i] = (on && kp[i]) ? __ldg(reinterpret_cast<const float4*>(kp[i] + ld_c * PJ_KC)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                if (on && ++ld_c == n_my) ld_c = 0;
-                return;
-            }
-            const int64_t k = (int64_t)(c0 + (c + rot) % n_my) * PJ_KC + kb * 4;    // (c >= n_my: not loaded, see below)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (rowp[i] && c < n_my) {
-                    if (p.vec_ok && k + 3 < p.F) v = __ldg(reinterpret_cast<const float4*>(rowp[i] + k));
-                    else {
-                        if (k + 0 < p.F) v.x = __ldg(rowp[i] + k + 0);
-                        if (k + 1 < p.F) v.y = __ldg(rowp[i] + k + 1);
-                        if (k + 2 < p.F) v.z = __ldg(rowp[i] + k + 2);
-                        if (k + 3 < p.F) v.w = __ldg(rowp[i] + k + 3);
-                    }
-                }
-                x[i] = v;
-            }
-        };
-        // Two register rings of PJ_DEPTH chunks each: while one is converted the other is in flight.  A ring is (re)filled
-        // in one burst, so a row is visited once per PJ_DEPTH chunks for PJ_DEPTH x 128 contiguous bytes -- with a
-        // power-of-two row pitch (F = 4096: 16 KB) the 128 rows of a tile sit in the same HBM bank, every visit is a row
-        // activate, and 128-byte visits serialise on the bank (measured: 4.5 us load latency at 20 % of peak bandwidth).
-        float4 ringA[PJ_DEPTH][4], ringB[PJ_DEPTH][4];
-        int s = 0;                                                    // smem stage of the next chunk, and its parity
-        uint32_t par = 1;
-        auto fill = [&](int cbase, float4 (&ring)[PJ_DEPTH][4]) {
-#pragma unroll
-            for (int q = 0; q < PJ_DEPTH; ++q) load_chunk(cbase + q, ring[q]);
-        };
-        auto drain = [&](int cbase, float4 (&ring)[PJ_DEPTH][4]) {
-#pragma unroll
-            for (int q = 0; q < PJ_DEPTH; ++q) {
-                if (cbase + q < n_my) {
-                    mbar_wait(bar + (16 + s) * 8, par);
-                    uint8_t* st = smem + s * L.stage_bytes;
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const int r = (t >> 3) + 32 * i;
-                        const uint32_t off = kb * PJ_LBO_A + (r >> 3) * 128 + (r & 7) * 16;
-                        float4 h, l;
-                        split_tf32_trunc(ring[q][i].x, h.x, l.x); split_tf32_trunc(ring[q][i].y, h.y, l.y);
-                        split_tf32_trunc(ring[q][i].z, h.z, l.z); split_tf32_trunc(ring[q][i].w, h.w, l.w);
-                        *reinterpret_cast<float4*>(st + L.a0 + off) = h;
-                        *reinterpret_cast<float4*>(st + L.a0 + PJ_A_BYTES + off) = l;
-                    }
-                    fence_proxy_async();                              // generic-proxy stores -> visible to the MMA's async reads
-                    mbar_arrive(bar + s * 8);
-                    if (++s == p.stages) { s = 0; par ^= 1; }
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (rowp[i] && c < n_my) {
+                if (p.vec_ok && k + 3 < p.F) v = __ldg(reinterpret_cast<const float4*>(rowp[i] + k));
+                else {
+                    if (k + 0 < p.F) v.x = __ldg(rowp[i] + k + 0);
+                    if (k + 1 < p.F) v.y = __ldg(rowp[i] + k + 1);
+                    if (k + 2 < p.F) v.z = __ldg(rowp[i] + k + 2);
+                    if (k + 3 < p.F) v.w = __ldg(rowp[i] + k + 3);
                 }
             }
-        };
-        fill(0, ringA);
-        for (int cb = 0; cb < n_my; cb += 2 * PJ_DEPTH) {
-            fill(cb + PJ_DEPTH, ringB);
-            drain(cb, ringA);
-            fill(cb + 2 * PJ_DEPTH, ringA);
-            drain(cb + PJ_DEPTH, ringB);
+            x[i] = v;
         }
-        // ---------------- epilogue: partial tile of this K split
-        if (n_my > 0 && warp < 6) {
-            mbar_wait(bar + 24 * 8, 0);
-            fence_after_sync();
-            const int q = warp & 3;
-            const int64_t row = (int64_t)tile * PJ_M + q * 32 + lane;
-            float* dst = p.partial + ((int64_t)sp * p.rows_padded + row) * p.N;
-            for (int c8 = 0; c8 < p.N / 32; ++c8) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + c8 * 32, v);
-                tmem_ld_wait();
+    };
+    // MMA side: descriptors built once, per instruction only the address field (16-byte units) moves
+    const uint32_t LBO_B = (uint32_t)(N / 8) * 128;
+    const uint64_t a_hi0 = smem_desc(sbase + L.a0 + g * 1024, PJ_LBO_A, 128), a_lo0 = smem_desc(sbase + L.a0 + PJ_A_BYTES + g * 1024, PJ_LBO_A, 128);
+    const uint64_t b_hi0 = smem_desc(sbase + L.b0, LBO_B, 128), b_lo0 = smem_desc(sbase + L.b0 + L.b_bytes, LBO_B, 128);
+    const uint64_t ka = (2 * PJ_LBO_A) >> 4, kbs = (2 * LBO_B) >> 4;
+    float acc[N / 2];
 #pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    reinterpret_cast<float4*>(dst + c8 * 32)[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                                              __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    uint32_t first = 0;
+    int prev = 0;
+    // Two register rings of PJ_DEPTH chunks each: while one is converted the other is in flight.  A ring is (re)filled
+    // in one burst, so a row is visited once per PJ_DEPTH chunks for PJ_DEPTH x 128 contiguous bytes -- with a
+    // power-of-two row pitch (F = 4096: 16 KB) the 128 rows of a tile sit in the same HBM bank, every visit is a row
+    // activate, and short visits serialise on the bank.
+    float4 ringA[PJ_DEPTH][4], ringB[PJ_DEPTH][4];
+    int s = 0;                                                    // smem stage of the next chunk, and its "empty" parity
+    uint32_t par = 1;
+    int done = 0;                                                 // chunks issued to the tensor cores
+    auto fill = [&](int cbase, float4 (&ring)[PJ_DEPTH][4]) {
+#pragma unroll
+        for (int q = 0; q < PJ_DEPTH; ++q) load_chunk(cbase + q, ring[q]);
+    };
+    auto drain = [&](int cbase, float4 (&ring)[PJ_DEPTH][4]) {
+#pragma unroll
+        for (int q = 0; q < PJ_DEPTH; ++q) {
+            if (cbase + q < n_my) {
+                mbar_wait(bar + (16 + s) * 8, par);
+                uint8_t* st = smem + s * L.stage_bytes;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int r = (t >> 3) + 32 * i;
+                    const uint32_t off = kb * PJ_LBO_A + (r >> 3) * 128 + (r & 7) * 16;
+                    float4 h, l;
+                    split_tf32_trunc(ring[q][i].x, h.x, l.x); split_tf32_trunc(ring[q][i].y, h.y, l.y);
+                    split_tf32_trunc(ring[q][i].z, h.z, l.z); split_tf32_trunc(ring[q][i].w, h.w, l.w);
+                    *reinterpret_cast<float4*>(st + L.a0 + off) = h;
+                    *reinterpret_cast<float4*>(st + L.a0 + PJ_A_BYTES + off) = l;
+                }
+                fence_proxy_async();                              // generic-proxy stores -> visible to the MMA's async reads
+                mbar_arrive(bar + s * 8);
+                // the whole stage (both warpgroups' rows, the weight slab) -> this warpgroup's 64 rows
+                mbar_wait(bar + s * 8, par ^ 1);
+                mbar_wait(bar + (8 + s) * 8, par ^ 1);
+                const uint64_t st_off = (uint64_t)(s * L.stage_bytes) >> 4;
+                uint64_t a_hi = a_hi0 + st_off, a_lo = a_lo0 + st_off, b_hi = b_hi0 + st_off, b_lo = b_lo0 + st_off;
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < PJ_KC / 8; ++j) {
+                    wgmma_tf32<N>(acc, a_hi, b_hi, first);
+                    first = 1;
+                    wgmma_tf32<N>(acc, a_lo, b_hi, 1);
+                    wgmma_tf32<N>(acc, a_hi, b_lo, 1);
+                    a_hi += ka; a_lo += ka; b_hi += kbs; b_lo += kbs;
+                }
+                wgmma_commit();
+                if (done++ > 0) {                                 // the previous chunk's group is done -> its stage goes back
+                    wgmma_wait<1>();
+                    warp_arrive(bar + (16 + prev) * 8);
+                }
+                prev = s;
+                if (++s == p.stages) { s = 0; par ^= 1; }
             }
         }
+    };
+    fill(0, ringA);
+    for (int cb = 0; cb < n_my; cb += 2 * PJ_DEPTH) {
+        fill(cb + PJ_DEPTH, ringB);
+        drain(cb, ringA);
+        fill(cb + 2 * PJ_DEPTH, ringA);
+        drain(cb + PJ_DEPTH, ringB);
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, tmem_cols);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    // ---------------- epilogue: partial tile of this K split, straight from the accumulator registers
+    const int w = (t >> 5) & 3;
+    const int64_t row0 = (int64_t)tile * PJ_M + g * 64 + w * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float* dst = p.partial + ((int64_t)sp * p.rows_padded + row0 + 8 * h) * N + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j)
+            *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    }
 }
 
 // Y[r, :] = sum over K splits of partial[s, r, :d] + bias, optional row L2 normalisation.  One warp per row.
@@ -329,13 +320,27 @@ int project_tc(int64_t n_out, const int64_t* idx, const float* table, int64_t F,
         int dev = 0;
         MMREC_CUDA(cudaGetDevice(&dev));
         if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
             if (dev >= 0 && dev < 64) attr_set[dev] = true;
         }
     }
-    if (p.vec_ok && (F % PJ_KC) == 0) project_tc_kernel<true><<<(unsigned)(P.n_tiles * P.n_splits), PJ_THREADS, L.total, stream>>>(p);
-    else project_tc_kernel<false><<<(unsigned)(P.n_tiles * P.n_splits), PJ_THREADS, L.total, stream>>>(p);
+    const bool fast = p.vec_ok && (F % PJ_KC) == 0;
+    const unsigned grid = (unsigned)(P.n_tiles * P.n_splits);
+    if (P.N == 64) {
+        if (fast) project_tc_kernel<64, true><<<grid, PJ_THREADS, L.total, stream>>>(p);
+        else project_tc_kernel<64, false><<<grid, PJ_THREADS, L.total, stream>>>(p);
+    } else if (P.N == 128) {
+        if (fast) project_tc_kernel<128, true><<<grid, PJ_THREADS, L.total, stream>>>(p);
+        else project_tc_kernel<128, false><<<grid, PJ_THREADS, L.total, stream>>>(p);
+    } else {
+        if (fast) project_tc_kernel<256, true><<<grid, PJ_THREADS, L.total, stream>>>(p);
+        else project_tc_kernel<256, false><<<grid, PJ_THREADS, L.total, stream>>>(p);
+    }
     MMREC_LAUNCH_CHECK();
     project_reduce_kernel<<<(unsigned)((n_out + 7) / 8), 256, 0, stream>>>(n_out, d, P.N, P.n_splits, P.rows_padded, partial, bias,
                                                                          l2_normalize, Y, ldy);

@@ -3,7 +3,7 @@
 //
 // Two arithmetic paths share the entry points:
 //   * exact fp32 on CUDA cores (gemm_simt.cuh): one fmaf chain per score, k ascending -- bit-faithful;
-//   * tcgen05 tensor cores with the 3xTF32 split (score_tc.cu) when the shape fits its tiles; selected by
+//   * wgmma tensor cores with the 3xTF32 split (score_tc.cu) when the shape fits its tiles; selected by
 //     mmrec_score_set_path() / env MMREC_SCORE_PATH = "simt" | "tc" (default: tc where supported).
 // mmrec_score_topk_f32 processes the users in row blocks whose score block stays L2-resident
 // (B_blk x n_items x 4 B <= 64 MiB), so the B x n_items matrix the reference materialises in HBM
@@ -31,9 +31,9 @@ int64_t score_cf_fallback_rows(const void* ws, int64_t B, int64_t n_items, int d
 int mask_apply(int64_t mask_nnz, const int64_t* mask_rows, const int64_t* mask_cols, int64_t row0, int64_t B,
                int64_t n_items, int64_t item_offset, float* S, int64_t ldS, cudaStream_t stream);
 
-// -1 unset | 0 simt: exact fp32 CUDA cores | 1 tc: tcgen05 GEMM -> L2-resident score block -> mask -> streaming top-k
+// -1 unset | 0 simt: exact fp32 CUDA cores | 1 tc: wgmma GEMM -> L2-resident score block -> mask -> streaming top-k
 //  2 auto (default): fused wherever its shape rules allow (enough item groups for the certified threshold), else tc
-//  3 fused: the certified-filter path of score_cf.cu (tcgen05 tf32 filter + exact fp32 finalists, no score matrix at all)
+//  3 fused: the certified-filter path of score_cf.cu (wgmma f16 filter + exact fp32 finalists, no score matrix at all)
 static int g_score_path = -1;
 static int score_path() {
     if (g_score_path < 0) {

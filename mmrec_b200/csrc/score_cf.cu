@@ -1,7 +1,7 @@
 // K3: full-catalog scoring fused with mask + top-k as a CERTIFIED FILTER on the tensor cores.
 //
 // The score matrix (115 MB per 4096 users at 7k items, 16 GB at 1M) is never written and no threshold depends on
-// timing.  The tensor cores (tcgen05, kind::f16, ONE pass over operands rounded to fp16 after a power-of-two scaling:
+// timing.  The tensor cores (wgmma f16, ONE pass over operands rounded to fp16 after a power-of-two scaling:
 // the same 11-bit significand as tf32 at twice the MMA rate and half the operand bytes) compute APPROXIMATE scores
 // s~ with a proven bound |s~ - s| <= eps * |u| * max|i| (+ a subnormal term that only matters for degenerate
 // tables, see cf_thr_kernel); they are only used to decide which (user, item) pairs can
@@ -9,14 +9,14 @@
 // kernel below), and the final order is taken on those fp32 values -- so the result is the fp32 top-k, tie -> lower
 // item index, exactly the contract of topk.cu.
 //
-//   cf_pack_kernel      operands -> fp16 (round to nearest) in the UMMA canonical K-major no-swizzle layout, tiles of
+//   cf_pack_kernel      operands -> fp16 (round to nearest) in the canonical K-major no-swizzle layout of wgmma, tiles of
 //                       128 rows, scaled by a power of two (per user row; one for the whole catalogue) so that the
 //                       largest element lands in [2^14, 2^15): no overflow, and fp16 subnormals only for elements
 //                       2^-28 below the largest.  Scores, norms and thresholds of a row all live in that scaled domain
 //                       (the exact re-scoring reads the original tables).  Row norms (users) / maximum row norm
 //                       (catalogue).  The catalogue side is packed once per embedding table (mmrec_catalog_pack_f32).
 //   cf_pass_kernel<1>   s~ for every (user, item); epilogue = maximum of every group of w = 16 gw consecutive items
-//                       (tcgen05.ld -> FMNMX3 tree), written as gmax[row][group].  No branches, no atomics.
+//                       (accumulator registers -> max tree -> quad shuffles), written as gmax[row][group].  No atomics.
 //   cf_thr_kernel       per row: t = the need-th largest group maximum, need = k + (masked items of the row).  At
 //                       least `need` distinct items have s~ >= t, so >= k unmasked ones have s >= t - eps'; hence every
 //                       member of the true top-k has s~ >= thr = t - 2 eps'.
@@ -29,8 +29,9 @@
 // Work distribution of the passes: a unit = (pair of 128-user tiles, 128-item tile); the units are dealt to the CTAs
 // (one per SM) in contiguous runs, so every SM gets the same number of units whatever the batch size (no wave
 // quantisation), a 256-user operand stays resident while its run of item tiles streams through a bulk-copy ring, and
-// every item slab read from L2 feeds two MMAs (32 B/cycle/SM at full tensor rate; one 128-user tile per CTA would
-// need 64, more than L2 delivers to 148 SMs).
+// every item slab read from L2 feeds two warpgroups' MMAs (one 128-user tile per CTA would need twice the L2 bandwidth
+// per flop).  Each pass kernel: warpgroup h = 0 / 1 owns user half h of the pair (wgmma M64 N128 K16 twice per K step:
+// 2 x 64 fp32 accumulator registers per thread) and runs the epilogue on its registers; warp 8 is the bulk-copy producer.
 #include <climits>
 #include <cstdio>
 #include <cstdlib>
@@ -42,10 +43,10 @@ namespace mmrec {
 
 using namespace tc;
 
-constexpr int CF_TILE = 128;                    // rows of one MMA operand tile (users: TMEM lanes; items: TMEM columns)
+constexpr int CF_TILE = 128;                    // rows of one operand tile (users: one warpgroup; items: the MMA's N)
 // An item slab is the whole K of a 128-item tile (8 / 16 / 32 KB at KP = 32 / 64 / 128): one barrier round trip per unit.
-constexpr int CF_EPI_WARPS = 16;                // (buffer parity, user half, TMEM lane quarter)
-constexpr int CF_THREADS = 64 + 32 * CF_EPI_WARPS;
+constexpr int CF_CONSUMER_WARPS = 8;            // two warpgroups, one per user half of the pair
+constexpr int CF_THREADS = 32 * CF_CONSUMER_WARPS + 32;
 constexpr int CF_MAX_STAGES = 10;
 constexpr int CF_CAP = 512;                     // candidates one warp ranks per row
 constexpr int CF_EX_SLOTS = 128;                // CTAs (and key buffers) of the exact kernel
@@ -53,7 +54,7 @@ constexpr float CF_EPS = 1.125f / 1024.f;       // |s~ - s| <= CF_EPS |u| |i|: t
 constexpr float CF_EPS_SUB = 1.0f / 16777216.f; // fp16 subnormal spacing 2^-24 (scaled domain): |dx| <= 2^-11 |x| + 2^-25 per element
 
 struct CfSmem {
-    uint32_t a, slab0, slab, bars, tmem_ptr, total;
+    uint32_t a, slab0, slab, bars, total;
     int stages;
 };
 __host__ __device__ inline CfSmem cf_smem(int KP) {
@@ -65,12 +66,11 @@ __host__ __device__ inline CfSmem cf_smem(int KP) {
     L.stages = (int)((226u * 1024u - L.slab0 - 300u) / slab);        // as many slabs in flight as shared memory holds
     if (L.stages > CF_MAX_STAGES) L.stages = CF_MAX_STAGES;
     L.bars = L.slab0 + L.stages * slab;
-    L.tmem_ptr = L.bars + 32 * 8;
-    L.total = L.tmem_ptr + 16;
+    L.total = L.bars + 32 * 8;
     return L;
 }
-// barrier slots
-enum { CB_AFULL = 0, CB_AFREE = 1, CB_FULL = 2, CB_EMPTY = 2 + CF_MAX_STAGES, CB_TFULL = 2 + 2 * CF_MAX_STAGES, CB_TEMPTY = 4 + 2 * CF_MAX_STAGES };
+// barrier slots: AFULL (tx) | AFREE (one arrival per consumer warp) | FULL[s] (tx) | EMPTY[s] (one arrival per consumer warp)
+enum { CB_AFULL = 0, CB_AFREE = 1, CB_FULL = 2, CB_EMPTY = 2 + CF_MAX_STAGES, CB_END = 2 + 2 * CF_MAX_STAGES };
 
 struct CfParams {
     const char* Upk;                            // fp16 [pairs][2][KP/8][16][8][8]
@@ -79,67 +79,8 @@ struct CfParams {
     int64_t B, n_items, n_units;
     float* gmax; int G, gw;                     // pass 1: [B][G], G = n_it * (8 / gw)
     const float* thr; uint4* bitmap;            // pass 2: [B], [B][n_it]
-    int dbg;                                    // tuning aid (env MMREC_CF_DEBUG): 1 = epilogue skips its TMEM loads, 2 = no MMAs issued
+    int dbg;                                    // tuning aid (env MMREC_CF_DEBUG): 2 = no MMAs issued, 16 = no item traffic
 };
-
-__device__ __forceinline__ void cf_tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr) : "memory");
-}
-// wait for the outstanding tcgen05.ld of this thread; the registers are operands so that no use of them can be
-// scheduled above the wait
-__device__ __forceinline__ void cf_tmem_wait16(uint32_t (&v)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                   "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])
-                 :: "memory");
-}
-__device__ __forceinline__ void cf_tmem_ld32(uint32_t taddr, uint32_t (&a)[16], uint32_t (&b)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]),
-          "=r"(a[8]), "=r"(a[9]), "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15]),
-          "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]), "=r"(b[4]), "=r"(b[5]), "=r"(b[6]), "=r"(b[7]),
-          "=r"(b[8]), "=r"(b[9]), "=r"(b[10]), "=r"(b[11]), "=r"(b[12]), "=r"(b[13]), "=r"(b[14]), "=r"(b[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void cf_tmem_wait32(uint32_t (&a)[16], uint32_t (&b)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3]), "+r"(a[4]), "+r"(a[5]), "+r"(a[6]), "+r"(a[7]),
-                   "+r"(a[8]), "+r"(a[9]), "+r"(a[10]), "+r"(a[11]), "+r"(a[12]), "+r"(a[13]), "+r"(a[14]), "+r"(a[15]),
-                   "+r"(b[0]), "+r"(b[1]), "+r"(b[2]), "+r"(b[3]), "+r"(b[4]), "+r"(b[5]), "+r"(b[6]), "+r"(b[7]),
-                   "+r"(b[8]), "+r"(b[9]), "+r"(b[10]), "+r"(b[11]), "+r"(b[12]), "+r"(b[13]), "+r"(b[14]), "+r"(b[15])
-                 :: "memory");
-}
-__device__ __forceinline__ float cf_max3(float a, float b, float c) {
-    float r;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-    return r;
-}
-__device__ __forceinline__ float cf_max16(const uint32_t (&v)[16]) {
-#define CF_F(i) __uint_as_float(v[i])
-    const float a = cf_max3(CF_F(0), CF_F(1), CF_F(2)), b = cf_max3(CF_F(3), CF_F(4), CF_F(5)), c = cf_max3(CF_F(6), CF_F(7), CF_F(8));
-    const float d = cf_max3(CF_F(9), CF_F(10), CF_F(11)), e = cf_max3(CF_F(12), CF_F(13), CF_F(14));
-    return fmaxf(cf_max3(a, b, c), cf_max3(d, e, CF_F(15)));
-#undef CF_F
-}
-// 16 scores -> 16 bits, bit (15 - j) = (v[j] < thr): sign of the (exact, Sterbenz) difference, shifted in by a funnel
-// shift -- FADD on the fma pipe, SHF on the alu pipe, two chains for ILP
-__device__ __forceinline__ uint32_t cf_lt16(const uint32_t (&v)[16], float thr) {
-    uint32_t a = 0, b = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        a = __funnelshift_l(__float_as_uint(__uint_as_float(v[j]) - thr), a, 1);
-        b = __funnelshift_l(__float_as_uint(__uint_as_float(v[8 + j]) - thr), b, 1);
-    }
-    return ((a & 0xffu) << 8) | (b & 0xffu);
-}
 
 // ---- producer: the 256-user operand of the current pair, then its run of item slabs ----------------------------
 __device__ __forceinline__ void cf_producer(const CfParams& p, const CfSmem& L, uint32_t sbase, int64_t u0, int64_t u1) {
@@ -176,159 +117,111 @@ __device__ __forceinline__ void cf_producer(const CfParams& p, const CfSmem& L, 
     }
 }
 
-// ---- MMA issuer: one thread, M128 N128 K16 (kind::f16), two user halves per item slab ------------------------------
-__device__ __forceinline__ void cf_mma(const CfParams& p, const CfSmem& L, uint32_t sbase, uint32_t tmem_base, int64_t u0, int64_t u1) {
+// ---- consumer warpgroup h: MMAs of user half h of the pair for each unit, then the epilogue on the registers ---------
+template <int PASS, int GPT>
+__device__ __forceinline__ void cf_consumer(const CfParams& p, const CfSmem& L, uint32_t sbase, int64_t u0, int64_t u1, int h) {
     const uint32_t bar = sbase + L.bars;
     constexpr uint32_t LBO = (CF_TILE / 8) * 128, SBO = 128;         // both operands: tiles of 128 rows
-    const uint32_t idesc = idesc_f16(CF_TILE, CF_TILE);
     const int ksteps = p.KP / 16;
     const uint32_t half_bytes = CF_TILE * p.KP * 2;
-    uint32_t a_cnt = 0;
-    int halves = 2;
-    // The issuing thread is a single instruction stream: measured (tools/probe_mma.py) ~200 cycles per tcgen05.mma when
-    // the descriptors are rebuilt around every instruction -- twice what the tensor pipe needs for M128 N128.  So the
-    // descriptors are built once and only their address field (low word, 16-byte units) moves.
-    const uint64_t a_desc0 = smem_desc(sbase + L.a, LBO, SBO), a_desc1 = smem_desc(sbase + L.a + half_bytes, LBO, SBO);
+    const int t = threadIdx.x & 127, w = t >> 5, lane = t & 31, q = lane & 3;
+    // descriptors are built once and only their address field (low word, 16-byte units) moves; rows 64..127 of the half
+    // start 8 core-matrix rows (1024 B) further
+    const uint64_t a_desc0 = smem_desc(sbase + L.a + h * half_bytes, LBO, SBO), a_desc1 = smem_desc(sbase + L.a + h * half_bytes + 1024, LBO, SBO);
     const uint64_t b_desc0 = smem_desc(sbase + L.slab0, LBO, SBO);
     const uint64_t kstep = (2 * LBO) >> 4;                           // one K step of 16 = two 16-byte k blocks
+    const uint64_t slab_step = L.slab >> 4;
+    float acc0[64], acc1[64];                                         // rows 16 w + lane / 4 (+ 8) and 64 + the same
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }   // (read by no MMA: the first K step overwrites)
     int64_t pair = u0 / p.n_it;
     int it = (int)(u0 - pair * p.n_it);
-    bool new_pair = true;
-    uint32_t slot = 0, ph = 0, buf = 0, tph = 1;                      // ring position / parity; accumulator buffer / its "empty" parity
+    bool new_pair = true, live = false;
+    uint32_t a_cnt = 0, slot = 0, ph = 0;
     uint64_t bd_slot = b_desc0;
-    const uint64_t slab_step = L.slab >> 4;
+    int64_t row0 = 0;                                                 // row of accumulator row r = 2 m + e2: row0 + 64 m + 8 e2
+    float thr[4];
     for (int64_t u = u0; u < u1; ++u) {
-        mbar_wait(bar + (CB_TEMPTY + buf) * 8, tph);                  // accumulators drained by the epilogue
         if (new_pair) {
             mbar_wait(bar + CB_AFULL * 8, a_cnt & 1);
             ++a_cnt;
-            halves = (pair * 2 * CF_TILE + CF_TILE < p.B) ? 2 : 1;
+            const int64_t base = pair * (2 * CF_TILE) + h * CF_TILE;
+            live = base < p.B;                                        // (a whole half beyond the batch: no MMAs, no output)
+            row0 = base + 16 * w + (lane >> 2);
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int64_t rr = row0 + 64 * (r >> 1) + 8 * (r & 1);
+                if (PASS == 2) thr[r] = rr < p.B ? __ldg(p.thr + rr) : INFINITY;
+            }
             new_pair = false;
         }
         mbar_wait(bar + (CB_FULL + slot) * 8, ph);
-        if (!(p.dbg & 64)) fence_after_sync();
-        const uint32_t d0 = tmem_base + (buf * 2 + 0) * CF_TILE, d1 = d0 + CF_TILE;
-        uint64_t ad0 = a_desc0, ad1 = a_desc1, bd = bd_slot;
-        if (!(p.dbg & 2)) {
-            if (halves == 2) {
+        if (live && !(p.dbg & 2)) {
+            uint64_t ad0 = a_desc0, ad1 = a_desc1, bd = bd_slot;
+            wgmma_fence();
 #pragma unroll 4
-                for (int j = 0; j < ksteps; ++j) {
-                    mma_f16(d0, ad0, bd, idesc, j ? 1u : 0u);
-                    mma_f16(d1, ad1, bd, idesc, j ? 1u : 0u);
-                    ad0 += kstep; ad1 += kstep; bd += kstep;
-                }
-            } else {
-#pragma unroll 4
-                for (int j = 0; j < ksteps; ++j) {
-                    mma_f16(d0, ad0, bd, idesc, j ? 1u : 0u);
-                    ad0 += kstep; bd += kstep;
-                }
+            for (int j = 0; j < ksteps; ++j) {
+                wgmma_f16<CF_TILE>(acc0, ad0, bd, j ? 1u : 0u);
+                wgmma_f16<CF_TILE>(acc1, ad1, bd, j ? 1u : 0u);
+                ad0 += kstep; ad1 += kstep; bd += kstep;
             }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc0);
+            wgmma_fence_regs(acc1);
         }
-        if (p.dbg & 32) {                                             // (tuning aid, only meaningful without MMAs: plain arrives)
-            mbar_arrive(bar + (CB_EMPTY + slot) * 8);
-            mbar_arrive(bar + (CB_TFULL + buf) * 8);
-        } else {
-            mma_commit(bar + (CB_EMPTY + slot) * 8);                  // slab consumed -> slot back to the producer
-            mma_commit(bar + (CB_TFULL + buf) * 8);                   // accumulators complete -> epilogue
-        }
+        warp_arrive(bar + (CB_EMPTY + slot) * 8);                     // slab consumed -> slot back to the producer
         bd_slot += slab_step;
         if (++slot == (uint32_t)L.stages) { slot = 0; ph ^= 1; bd_slot = b_desc0; }
+        const int cur_it = it;
         if (++it == p.n_it) { it = 0; ++pair; new_pair = true; }
-        if (new_pair || u + 1 == u1) mma_commit(bar + CB_AFREE * 8);
-        buf ^= 1;
-        if (buf == 0) tph ^= 1;
-    }
-}
-
-// ---- epilogue: thread = one user row, 128 accumulator columns per unit in 8 chunks of 16, loads one chunk ahead --------
-template <int PASS, int GPT>
-__device__ __forceinline__ void cf_epilogue(const CfParams& p, const CfSmem& L, uint32_t sbase, uint32_t tmem_base, int u0, int u1,
-                                            int e, int lane) {
-    const uint32_t bar = sbase + L.bars;
-    const int q = (e + 2) & 3;                                       // = warp % 4: the TMEM lane quarter this warp may read
-    const int h = (e >> 2) & 1, par = e >> 3;
-    constexpr int gpt = GPT;                                          // groups per item tile (pass 1): 8 / gw
-    int cur_pair = -1;
-    int64_t row = 0;
-    bool live = false;
-    float thr = INFINITY;
-    int pair = (u0 + par) / p.n_it;
-    int it = (u0 + par) - pair * p.n_it;
-    uint32_t fph = 0;
-    for (int u = u0 + par; u < u1; u += 2, fph ^= 1) {
-        if (pair != cur_pair) {
-            cur_pair = pair;
-            row = (int64_t)pair * (2 * CF_TILE) + h * CF_TILE + q * 32 + lane;
-            live = row < p.B;
-            if (PASS == 2) thr = live ? __ldg(p.thr + row) : INFINITY;
-        }
-        mbar_wait(bar + (CB_TFULL + par) * 8, fph);
-        fence_after_sync();
-        // (a whole half beyond the batch: nothing to read, but the buffer still has to be released)
-        if ((int64_t)pair * (2 * CF_TILE) + h * CF_TILE < p.B && !(p.dbg & 1)) {
-            const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + (par * 2 + h) * CF_TILE;
-            const int n_valid = (int)(p.n_items - (int64_t)it * CF_TILE);      // < 128 on the last tile only
-            uint32_t va[16], vb[16];
-            float gm[8];
-            uint32_t w[4];
+        if (new_pair || u + 1 == u1) warp_arrive(bar + CB_AFREE * 8);  // this warp is done with the pair's user operand
+        if (!live) continue;
+        // ---- epilogue, one accumulator row at a time (r = 2 m + e2: set m, row half e2); columns >= n_valid (last item
+        // tile only) read as -inf: never a maximum, never a hit
+        const int n_valid = (int)(p.n_items - (int64_t)cur_it * CF_TILE);
 #pragma unroll
-            for (int c = 0; c < 8; c += 2) {
-                // 32 columns per tcgen05.ld (MMREC_CF_DEBUG bit 2: 16 per load, the next one requested before this one is used)
-                if (p.dbg & 4) {
-                    if (c == 0) cf_tmem_ld16(t0, va);
-                    cf_tmem_wait16(va);
-                    cf_tmem_ld16(t0 + (c + 1) * 16, vb);
-                } else {
-                    cf_tmem_ld32(t0 + c * 16, va, vb);
-                    cf_tmem_wait32(va, vb);
-                }
-                if (n_valid < CF_TILE) {
+        for (int r = 0; r < 4; ++r) {
+            const float* acc = r < 2 ? acc0 : acc1;
+            const int e2 = r & 1;
+            const int64_t row = row0 + 64 * (r >> 1) + 8 * e2;
+            auto val = [&](int j, int e) {                            // column 8 j + 2 q + e of the row
+                const float v = acc[4 * j + 2 * e2 + e];
+                return 8 * j + 2 * q + e < n_valid ? v : -INFINITY;
+            };
+            if (PASS == 1) {
+                // group of 16 columns = j = 2 g, 2 g + 1: this lane's 4 values, then the quad's maximum; wider groups fold
+                float gm[GPT];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (c * 16 + j >= n_valid) va[j] = 0xff800000u;          // -inf: never a maximum, never a hit
-                }
-                if (PASS == 1) gm[c] = cf_max16(va);
-                const uint32_t lt0 = PASS == 2 ? cf_lt16(va, thr) : 0u;
-                if (p.dbg & 4) {
-                    cf_tmem_wait16(vb);
-                    if (c + 2 < 8) cf_tmem_ld16(t0 + (c + 2) * 16, va);
-                }
-                if (n_valid < CF_TILE) {
+                for (int g = 0; g < GPT; ++g) {
+                    float m = -INFINITY;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if ((c + 1) * 16 + j >= n_valid) vb[j] = 0xff800000u;
+                    for (int j = g * (16 / GPT); j < (g + 1) * (16 / GPT); ++j) m = fmaxf(m, fmaxf(val(j, 0), val(j, 1)));
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+                    gm[g] = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
                 }
-                if (PASS == 1) {
-                    gm[c + 1] = cf_max16(vb);
-                    if (gpt <= 4) gm[c] = fmaxf(gm[c], gm[c + 1]);    // groups of 32 items and wider: fold as we go
-                    if (gpt == 8 && (c & 2) && live)                  // groups of 16: four maxima are a 16-byte store
-                        reinterpret_cast<float4*>(p.gmax + row * p.G + (int64_t)it * 8)[c >> 2] = make_float4(gm[c - 2], gm[c - 1], gm[c], gm[c + 1]);
+                if (row < p.B) {
+                    float* dst = p.gmax + row * p.G + (int64_t)cur_it * GPT;
+#pragma unroll
+                    for (int g = 0; g < GPT; ++g)
+                        if ((g & 3) == q) dst[g] = gm[g];
                 }
-                if (PASS == 2) w[c >> 1] = ~((lt0 << 16) | cf_lt16(vb, thr));   // bit (31 - j) of word (c / 2): column 32 (c / 2) + j passes
-            }
-            if (live) {
-                if (PASS == 1) {
-                    float* dst = p.gmax + row * p.G + (int64_t)it * gpt;
-                    if (gpt == 8) {
-                        // (stored inside the loop)
-                    } else if (gpt == 4) {
-                        *reinterpret_cast<float4*>(dst) = make_float4(gm[0], gm[2], gm[4], gm[6]);
-                    } else if (gpt == 2) {
-                        *reinterpret_cast<float2*>(dst) = make_float2(fmaxf(gm[0], gm[2]), fmaxf(gm[4], gm[6]));
-                    } else {
-                        *dst = fmaxf(fmaxf(gm[0], gm[2]), fmaxf(gm[4], gm[6]));
-                    }
-                } else {
-                    p.bitmap[row * p.n_it + it] = make_uint4(w[0], w[1], w[2], w[3]);
+            } else {
+                // bit (31 - c) of word b: column 32 b + c passes, s~ >= thr (the sign of the exact difference)
+                uint32_t wd[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e)
+                        if (!(__float_as_uint(val(j, e) - thr[r]) >> 31)) wd[j >> 2] |= 1u << (31 - (8 * (j & 3) + 2 * q + e));
+#pragma unroll
+                for (int b = 0; b < 4; ++b) {
+                    wd[b] |= __shfl_xor_sync(0xffffffffu, wd[b], 1);
+                    wd[b] |= __shfl_xor_sync(0xffffffffu, wd[b], 2);
                 }
+                if (q == r && row < p.B) p.bitmap[row * p.n_it + cur_it] = make_uint4(wd[0], wd[1], wd[2], wd[3]);
             }
         }
-        fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar + (CB_TEMPTY + par) * 8);
-        it += 2;
-        while (it >= p.n_it) { it -= p.n_it; ++pair; }
     }
 }
 
@@ -340,28 +233,23 @@ __global__ void __launch_bounds__(CF_THREADS, 1) cf_pass_kernel(const CfParams p
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t bar = sbase + L.bars;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < CB_TEMPTY; ++i) mbar_init(bar + i * 8, 1);
-        mbar_init(bar + CB_TEMPTY * 8, 8); mbar_init(bar + (CB_TEMPTY + 1) * 8, 8);   // 2 halves x 4 lane quarters release a buffer pair
+        mbar_init(bar + CB_AFULL * 8, 1);
+        mbar_init(bar + CB_AFREE * 8, CF_CONSUMER_WARPS);
+        for (int s = 0; s < CF_MAX_STAGES; ++s) {
+            mbar_init(bar + (CB_FULL + s) * 8, 1);
+            mbar_init(bar + (CB_EMPTY + s) * 8, CF_CONSUMER_WARPS);
+        }
         mbar_fence_init();
     }
-    if (warp == 1) { tmem_alloc(sbase + L.tmem_ptr, 512); tmem_relinquish(); }
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + L.tmem_ptr);
     // contiguous run of units for this CTA
     const int64_t u0 = (int64_t)blockIdx.x * p.n_units / gridDim.x;
     const int64_t u1 = (int64_t)(blockIdx.x + 1) * p.n_units / gridDim.x;
-    if (warp == 0) {
+    if (warp == CF_CONSUMER_WARPS) {
         if (lane == 0) cf_producer(p, L, sbase, u0, u1);
-    } else if (warp == 1) {
-        if (lane == 0) cf_mma(p, L, sbase, tmem_base, u0, u1);
     } else {
-        cf_epilogue<PASS, GPT>(p, L, sbase, tmem_base, (int)u0, (int)u1, warp - 2, lane);
+        cf_consumer<PASS, GPT>(p, L, sbase, u0, u1, warp >> 2);
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 // ------------------------------------------------------------------------------------------------------------------

@@ -1,18 +1,19 @@
-// K3 on the tensor cores: S = U I^T with tcgen05.mma (kind::tf32) and the 3xTF32 operand split
+// K3 on the tensor cores: S = U I^T with wgmma (tf32) and the 3xTF32 operand split
 //     u = u_hi + u_lo,  i = i_hi + i_lo   (each part exactly representable in tf32)
 //     <u, i> ~= u_hi.i_hi + u_lo.i_hi + u_hi.i_lo          (dropped term u_lo.i_lo ~ 2^-22 relative)
-// accumulated in fp32 in TMEM: fp32-level accuracy (the reference computes this GEMM in fp32 and the top-k
+// accumulated in fp32 registers: fp32-level accuracy (the reference computes this GEMM in fp32 and the top-k
 // order is not stable under single-pass TF32, BASELINE.md 2.3) at tensor-pipe speed.
 //
 // Data path
-//   pack kernels   split + re-tile both operands ONCE into the UMMA canonical K-major no-swizzle layout
+//   pack kernels   split + re-tile both operands ONCE into the canonical K-major no-swizzle layout of wgmma
 //                  (8 x 16 B core matrices), so a tile slab is a contiguous byte range in global memory;
 //   producer warp  cp.async.bulk (UBLKCP) global -> shared, completion on mbarriers; the 128-user tile (hi+lo)
-//                  stays resident, item tiles stream as 32 KB slabs (256 items x 32 k) through a 4-slot ring;
-//   MMA warp       one thread issues tcgen05.mma M128 N256 K8 into one of two 256-column TMEM accumulators and
-//                  frees ring slots / publishes accumulators with tcgen05.commit;
-//   epilogue       4 warps (one per TMEM lane quarter) read the accumulator with tcgen05.ld 32x32b.x32 and write
-//                  the scores (this file) or filter them into per-user candidate lists (score_fused.cu).
+//                  stays resident, item tiles stream as 32 KB slabs (256 items x 32 k) through a 3-4-slot ring;
+//   consumers      two warpgroups, 64 users each: wgmma M64 N256 K8 into 128 fp32 registers per thread; a slot goes
+//                  back to the producer once the wgmma group that read it has completed (one group kept in flight),
+//                  and the finished accumulator is written straight from the registers as scores.
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace mmrec {
@@ -28,7 +29,7 @@ struct ScoreTcParams {
 };
 
 struct TcSmemLayout {
-    uint32_t u_hi, u_lo, slab0, bars, tmem_ptr, total;
+    uint32_t u_hi, u_lo, slab0, bars, total;
     int stages;
 };
 __host__ __device__ inline TcSmemLayout tc_smem_layout(int KP) {
@@ -37,11 +38,11 @@ __host__ __device__ inline TcSmemLayout tc_smem_layout(int KP) {
     L.stages = KP >= 128 ? 3 : 4;
     L.u_hi = 0; L.u_lo = u_bytes; L.slab0 = 2 * u_bytes;
     L.bars = L.slab0 + L.stages * TC_SLAB_BYTES;
-    L.tmem_ptr = L.bars + 16 * 8;
-    L.total = L.tmem_ptr + 16;
+    L.total = L.bars + 16 * 8;
     return L;
 }
-// barrier slots: 0 u_full | 1..4 full[s] | 5..8 empty[s] | 9,10 tmem_full[b] | 11,12 tmem_empty[b]
+// barrier slots: 0 u_full | 1..4 full[s] | 5..8 empty[s] (one arrival per consumer warp)
+constexpr int TC_CONSUMER_WARPS = 8;
 
 __device__ __forceinline__ void tc_producer(const ScoreTcParams& p, const TcSmemLayout& L, uint32_t sbase, int ut, int it0, int it1) {
     const uint32_t bar = sbase + L.bars;
@@ -64,46 +65,70 @@ __device__ __forceinline__ void tc_producer(const ScoreTcParams& p, const TcSmem
     }
 }
 
-__device__ __forceinline__ void tc_mma_issuer(const ScoreTcParams& p, const TcSmemLayout& L, uint32_t sbase, uint32_t tmem_base,
-                                              int it0, int it1) {
+// consumer warpgroup g: users [64 g, 64 g + 64) of the tile, all 256 items of each item tile
+__device__ __forceinline__ void tc_consumer(const ScoreTcParams& p, const TcSmemLayout& L, uint32_t sbase, int ut, int it0, int it1, int g) {
     const uint32_t bar = sbase + L.bars;
     constexpr uint32_t LBO_A = (TC_M / 8) * 128, LBO_B = (TC_N / 8) * 128, SBO = 128;
-    const uint32_t idesc = idesc_tf32(TC_M, TC_N);
     const int kchunks = p.KP / TC_KC;
+    const int t = threadIdx.x & 127, w = t >> 5, lane = t & 31;
     mbar_wait(bar + 0 * 8, 0);
-    fence_after_sync();
-    // descriptors are built once; per instruction only the address field moves (see tools/probe_mma.py: rebuilding them
-    // around every MMA makes the issuing thread, not the tensor pipe, the limit)
-    const uint64_t a_hi0 = smem_desc(sbase + L.u_hi, LBO_A, SBO), a_lo0 = smem_desc(sbase + L.u_lo, LBO_A, SBO);
+    // descriptors are built once; per instruction only the address field moves
+    const uint64_t a_hi0 = smem_desc(sbase + L.u_hi + g * 1024, LBO_A, SBO), a_lo0 = smem_desc(sbase + L.u_lo + g * 1024, LBO_A, SBO);
     const uint64_t b0 = smem_desc(sbase + L.slab0, LBO_B, SBO);
     const uint64_t ka = (2 * LBO_A) >> 4, kb = (2 * LBO_B) >> 4, slab_step = TC_SLAB_BYTES >> 4;
-    uint32_t slot = 0, ph = 0;
+    const bool vec = ((p.ldS & 1) == 0) && ((((uintptr_t)p.S) & 7) == 0);
+    float acc[TC_N / 2];
+#pragma unroll
+    for (int i = 0; i < TC_N / 2; ++i) acc[i] = 0.f;
+    uint32_t slot = 0, ph = 0, prev = 0;
     uint64_t bd_slot = b0;
-    for (int it = it0, t = 0; it < it1; ++it, ++t) {
-        const uint32_t buf = t & 1;
-        mbar_wait(bar + (11 + buf) * 8, ((t >> 1) & 1) ^ 1);     // accumulator drained by the epilogue
-        fence_after_sync();
-        const uint32_t d_tmem = tmem_base + buf * TC_N;
-        uint32_t acc = 0;
+    for (int it = it0; it < it1; ++it) {
+        uint32_t first = 0;
         uint64_t a_hi = a_hi0, a_lo = a_lo0;
-        for (int c = 0; c < 2 * kchunks; ++c) {
+        // slab c: k chunk c % kchunks of the items' hi parts (c < kchunks: u_hi.i_hi + u_lo.i_hi) or lo parts (u_hi.i_lo)
+        auto slab = [&](int c, auto item_lo) {
             mbar_wait(bar + (1 + slot) * 8, ph);
-            fence_after_sync();
-            const bool item_lo = c >= kchunks;
-            if (c == kchunks) { a_hi = a_hi0; a_lo = a_lo0; }     // second sweep over K: the items' lo parts
             uint64_t bd = bd_slot;
+            wgmma_fence();
 #pragma unroll
             for (int j = 0; j < TC_KC / 8; ++j) {
-                mma_tf32(d_tmem, a_hi, bd, idesc, acc);
-                acc = 1;
-                if (!item_lo) mma_tf32(d_tmem, a_lo, bd, idesc, 1);
+                wgmma_tf32<TC_N>(acc, a_hi, bd, first);
+                first = 1;
+                if (!decltype(item_lo)::value) wgmma_tf32<TC_N>(acc, a_lo, bd, 1);
                 a_hi += ka; a_lo += ka; bd += kb;
             }
-            mma_commit(bar + (5 + slot) * 8);                     // slab consumed -> slot back to the producer
+            wgmma_commit();
+            if (c > 0) {                                          // the previous slab's group is done -> its slot goes back
+                wgmma_wait<1>();
+                warp_arrive(bar + (5 + prev) * 8);
+            }
+            prev = slot;
             bd_slot += slab_step;
             if (++slot == (uint32_t)L.stages) { slot = 0; ph ^= 1; bd_slot = b0; }
+        };
+        for (int c = 0; c < kchunks; ++c) slab(c, std::false_type());
+        a_hi = a_hi0; a_lo = a_lo0;                               // second sweep over K: the items' lo parts
+        for (int c = kchunks; c < 2 * kchunks; ++c) slab(c, std::true_type());
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        warp_arrive(bar + (5 + prev) * 8);
+        const int64_t row0 = (int64_t)ut * TC_M + g * 64 + w * 16 + (lane >> 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t row = row0 + 8 * h;
+            if (row >= p.B) continue;
+            float* dst = p.S + row * p.ldS;
+#pragma unroll
+            for (int j = 0; j < TC_N / 8; ++j) {
+                const int64_t col = (int64_t)it * TC_N + 8 * j + 2 * (lane & 3);
+                const float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
+                if (vec && col + 1 < p.n_items) *reinterpret_cast<float2*>(dst + col) = make_float2(x, y);
+                else {
+                    if (col < p.n_items) dst[col] = x;
+                    if (col + 1 < p.n_items) dst[col + 1] = y;
+                }
+            }
         }
-        mma_commit(bar + (9 + buf) * 8);                          // accumulator complete -> epilogue
     }
 }
 
@@ -114,59 +139,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) score_tc_kernel(const ScoreTcPa
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t bar = sbase + L.bars;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 11; ++i) mbar_init(bar + i * 8, 1);
-        mbar_init(bar + 11 * 8, 128); mbar_init(bar + 12 * 8, 128);
+        for (int i = 0; i < 5; ++i) mbar_init(bar + i * 8, 1);
+        for (int i = 5; i < 9; ++i) mbar_init(bar + i * 8, TC_CONSUMER_WARPS);
         mbar_fence_init();
     }
-    if (warp == 1) { tmem_alloc(sbase + L.tmem_ptr, 512); tmem_relinquish(); }
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + L.tmem_ptr);
 
     const int ut = blockIdx.x / p.n_splits, sp = blockIdx.x % p.n_splits;
     const int it0 = sp * p.tiles_per_split;
     const int it1 = min(p.n_itiles, it0 + p.tiles_per_split);
-
-    if (warp == 0) {
-        if (lane == 0 && it0 < it1) tc_producer(p, L, sbase, ut, it0, it1);
-    } else if (warp == 1) {
-        if (lane == 0 && it0 < it1) tc_mma_issuer(p, L, sbase, tmem_base, it0, it1);
+    if (it0 >= it1) return;
+    if (warp == TC_CONSUMER_WARPS) {
+        if (lane == 0) tc_producer(p, L, sbase, ut, it0, it1);
     } else {
-        const int q = warp & 3;                                   // TMEM lane quarter this warp may read
-        const int64_t row = (int64_t)ut * TC_M + q * 32 + lane;
-        const bool vec = ((p.ldS & 3) == 0) && ((((uintptr_t)p.S) & 15) == 0);
-        for (int it = it0, t = 0; it < it1; ++it, ++t) {
-            const uint32_t buf = t & 1;
-            mbar_wait(bar + (9 + buf) * 8, (t >> 1) & 1);
-            fence_after_sync();
-#pragma unroll 1
-            for (int c8 = 0; c8 < TC_N / 32; ++c8) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * TC_N + c8 * 32, v);
-                tmem_ld_wait();
-                const int64_t col0 = (int64_t)it * TC_N + c8 * 32;
-                if (row < p.B && col0 < p.n_items) {
-                    float* dst = p.S + row * p.ldS + col0;
-                    if (vec && col0 + 32 <= p.n_items) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            reinterpret_cast<float4*>(dst)[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                                            __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (col0 + j < p.n_items) dst[j] = __uint_as_float(v[j]);
-                    }
-                }
-            }
-            fence_before_sync();
-            mbar_arrive(bar + (11 + buf) * 8);
-        }
+        tc_consumer(p, L, sbase, ut, it0, it1, warp >> 2);
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 static inline int kp_of(int d) { return d <= 32 ? 32 : (d <= 64 ? 64 : 128); }
@@ -223,59 +210,62 @@ int score_tc(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int6
 
 }  // namespace mmrec
 
-// ---- measurement aid: how many cycles does one tcgen05.mma (cta_group::1, both operands in shared memory, K-major, no swizzle
-// -- the form every tensor-core kernel of this library issues) take when nothing else runs?  One CTA per SM, one thread
-// issues `iters` MMAs of M = 128, the given N and K = 32 bytes (8 tf32 / 16 bf16) into one accumulator, commits and waits.
+// ---- measurement aid: how many cycles does one wgmma (both operands in shared memory, K-major, no swizzle -- the form
+// every tensor-core kernel of this library issues) take when nothing else runs?  One CTA per SM, one warpgroup issues
+// `iters` wgmmas of M = 64, the given N and K = 32 bytes (8 tf32 / 16 bf16) into one accumulator, commits and waits.
 namespace mmrec {
-__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int kind, int N, int iters, int distinct, long long* __restrict__ cycles) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ uint32_t tmem_ptr_sm;
-    __shared__ __align__(8) unsigned long long bar_sm;
-    const uint32_t sbase = tc::smem_u32(smem);
-    const uint32_t bar = tc::smem_u32(&bar_sm);
-    for (int i = threadIdx.x; i < 48 * 1024; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0;   // 192 KB of zeros
-    if (threadIdx.x == 0) { tc::mbar_init(bar, 1); tc::mbar_fence_init(); }
-    if (threadIdx.x < 32) { tc::tmem_alloc(tc::smem_u32(&tmem_ptr_sm), 512); tc::tmem_relinquish(); }
-    tc::fence_proxy_async();
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_ptr_sm;
-    if (threadIdx.x == 0) {
-        const uint32_t LBO_A = (128 / 8) * 128, LBO_B = (uint32_t)(N / 8) * 128;
-        // instruction descriptors: tf32 (a/b format 2) or bf16 (format 1), fp32 accumulate, K-major both
-        const uint32_t idesc = kind == 0 ? tc::idesc_tf32(128, N)
-                                         : tc::idesc_bf16(128, N);
-        const long long t0 = clock64();
-        if (distinct == 0) {
-            // lean issue loop: descriptors built once, only the address field moves (8 K steps, unrolled)
-            const uint64_t a0 = tc::smem_desc(sbase, LBO_A, 128), b0 = tc::smem_desc(sbase + 65536, LBO_B, 128);
-            const uint64_t ka = (2 * LBO_A) >> 4, kb = (2 * LBO_B) >> 4;
-            for (int i = 0; i < iters; i += 8) {
-                uint64_t ad = a0, bd = b0;
+template <int N, int KIND>
+__device__ __forceinline__ long long mma_rate_run(int iters, int distinct, uint32_t sbase) {
+    constexpr uint32_t LBO_A = (64 / 8) * 128, LBO_B = (uint32_t)(N / 8) * 128;
+    float acc[N / 2];
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    if (kind == 0) tc::mma_tf32(tmem, ad, bd, idesc, (i | j) ? 1u : 0u);
-                    else tc::mma_f16(tmem, ad, bd, idesc, (i | j) ? 1u : 0u);
-                    ad += ka; bd += kb;
-                }
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    const long long t0 = clock64();
+    tc::wgmma_fence();
+    if (distinct == 0) {
+        // lean issue loop: descriptors built once, only the address field moves (8 K steps, unrolled)
+        const uint64_t a0 = tc::smem_desc(sbase, LBO_A, 128), b0 = tc::smem_desc(sbase + 65536, LBO_B, 128);
+        const uint64_t ka = (2 * LBO_A) >> 4, kb = (2 * LBO_B) >> 4;
+        for (int i = 0; i < iters; i += 8) {
+            uint64_t ad = a0, bd = b0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                if (KIND == 0) tc::wgmma_tf32<N>(acc, ad, bd, (i | j) ? 1u : 0u);
+                else tc::wgmma_bf16<N>(acc, ad, bd, (i | j) ? 1u : 0u);
+                ad += ka; bd += kb;
             }
-        } else
+        }
+    } else {
         for (int i = 0; i < iters; ++i) {
             const uint32_t off = (uint32_t)(i % distinct) * 2 * LBO_A;            // walk over `distinct` K steps of the operands
             const uint64_t ad = tc::smem_desc(sbase + off, LBO_A, 128);
             const uint64_t bd = tc::smem_desc(sbase + 65536 + (uint32_t)(i % distinct) * 2 * LBO_B, LBO_B, 128);
-            if (kind == 0) tc::mma_tf32(tmem, ad, bd, idesc, i > 0);
-            else tc::mma_f16(tmem, ad, bd, idesc, i > 0);
+            if (KIND == 0) tc::wgmma_tf32<N>(acc, ad, bd, i > 0);
+            else tc::wgmma_bf16<N>(acc, ad, bd, i > 0);
         }
-        tc::mma_commit(bar);
-        tc::mbar_wait(bar, 0);
-        const long long t1 = clock64();
-        cycles[blockIdx.x] = t1 - t0;
     }
-    tc::fence_before_sync();
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::wgmma_fence_regs(acc);
+    const long long t1 = clock64();
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) s += acc[i];
+    return (t1 - t0) + (s == 1234.5f ? 1 : 0);                        // (keeps the accumulators, hence the MMAs, alive)
+}
+
+__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int kind, int N, int iters, int distinct, long long* __restrict__ cycles) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const uint32_t sbase = tc::smem_u32(smem);
+    for (int i = threadIdx.x; i < 48 * 1024; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0;   // 192 KB of zeros
+    tc::fence_proxy_async();
     __syncthreads();
-    if (threadIdx.x < 32) tc::tmem_dealloc(tmem, 512);
+    long long c;
+    if (kind == 0) c = N == 64 ? mma_rate_run<64, 0>(iters, distinct, sbase)
+                               : (N == 128 ? mma_rate_run<128, 0>(iters, distinct, sbase) : mma_rate_run<256, 0>(iters, distinct, sbase));
+    else c = N == 64 ? mma_rate_run<64, 1>(iters, distinct, sbase)
+                     : (N == 128 ? mma_rate_run<128, 1>(iters, distinct, sbase) : mma_rate_run<256, 1>(iters, distinct, sbase));
+    if (threadIdx.x == 0) cycles[blockIdx.x] = c;
 }
 }  // namespace mmrec
 

@@ -1,11 +1,11 @@
-// Thin inline-PTX layer for the sm_100a tensor-core kernels: mbarrier, bulk async copy (UBLKCP), tcgen05
-// alloc / mma / commit / ld, UMMA shared-memory and instruction descriptors.  Encodings cross-checked against
-// the CUTLASS 4.x headers (cute/arch/mma_sm100_desc.hpp, mma_sm100_umma.hpp, copy_sm100.hpp) -- the kernels
-// themselves are hand-written.
+// Thin inline-PTX layer for the sm_90a tensor-core kernels: mbarrier, bulk async copy (UBLKCP), wgmma fence / commit /
+// wait and the wgmma shared-memory descriptor (the MMA wrappers themselves are in wgmma.cuh).  The descriptor encoding
+// follows the PTX ISA's "matrix descriptor" for wgmma -- the kernels are hand-written.
 #pragma once
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace mmrec {
 namespace tc {
@@ -32,8 +32,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
         : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug must trap within ~2 s of wall time, not hang the GPU (the box is shared and a hang
-// is a strike).  The clock is only consulted after the fast path failed a few thousand times.
+// Bounded wait: a protocol bug must trap within ~2 s of wall time, not hang the GPU.  The clock is only consulted after
+// the fast path failed a few thousand times.  (No printf here: a call inside a run of in-flight wgmmas makes ptxas
+// serialise them.)
 __device__ __forceinline__ uint64_t global_ns() {
     uint64_t t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -44,10 +45,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint64_t t0 = 0;
     while (!mbar_try_wait(bar, parity)) {
         if (++spins == 4096u) t0 = global_ns();
-        if (spins > 4096u && (spins & 1023u) == 0 && global_ns() - t0 > 2000000000ull) {
-            printf("mmrec: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-            __trap();
-        }
+        if (spins > 4096u && (spins & 1023u) == 0 && global_ns() - t0 > 2000000000ull) __trap();
     }
 }
 
@@ -57,53 +55,25 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
                  ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-// ---- tcgen05 ----------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
+// ---- wgmma (warpgroup MMA) ----------------------------------------------------------------------------------------
+// Every thread of the issuing warpgroup executes these.  wgmma_fence orders earlier register / shared-memory accesses
+// before the next wgmma; commit closes a group of issued wgmmas; wait_group<N> returns once at most N groups are in
+// flight, after which the accumulators of the completed groups may be read and their shared-memory operands reused.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the accumulators live across the wait: no read of them may be scheduled above it
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, kind::tf32, issued by ONE thread
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// the same with kind::f16 (fp16 or bf16 operands as the instruction descriptor says), K = 16 per instruction
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier once every previously issued MMA of this thread has completed
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 columns of fp32: thread i of the warp gets TMEM lane (base_lane + i), columns [col, col + 32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
+// one arrival per warp on `bar` once every lane of the warp is past this point (e.g. its wgmma reads are complete)
+__device__ __forceinline__ void warp_arrive(uint32_t bar) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
 // ---- descriptors --------------------------------------------------------------------------------------------
@@ -115,19 +85,8 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t smem_addr, uint32_t lbo_b
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= 1ull << 46;                    // descriptor version: Blackwell
-    return d;                           // base_offset 0, lbo_mode 0, layout_type 0 (SWIZZLE_NONE)
+    return d;                           // base_offset 0, layout_type 0 (no swizzle)
 }
-// instruction descriptor, kind::tf32, fp32 accumulate, both operands K-major
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// instruction descriptor, kind::f16 with fp16 operands (format 0; bf16 would be 1), fp32 accumulate, both operands K-major
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N) { return idesc_f16(M, N) | (1u << 7) | (1u << 10); }
 
 // 3xTF32 split: hi = x rounded to tf32 (RN, ties away), lo = (x - hi) rounded to tf32; x = hi + lo to ~2^-22 |x|
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
@@ -149,14 +108,14 @@ __device__ __forceinline__ void split_tf32_trunc(float x, float& hi, float& lo) 
 }  // namespace tc
 
 // ---- tile geometry shared by the tensor-core kernels ---------------------------------------------------------
-constexpr int TC_M = 128;          // users per CTA tile = TMEM lanes
-constexpr int TC_N = 256;          // items per accumulator = TMEM columns
+constexpr int TC_M = 128;          // users per CTA tile: two consumer warpgroups of 64 rows
+constexpr int TC_N = 256;          // items per accumulator (128 fp32 registers per thread)
 constexpr int TC_KC = 32;          // k per slab
 constexpr int TC_SLAB_BYTES = TC_N * TC_KC * 4;    // 32 KB
-constexpr int TC_THREADS = 192;    // warp 0 producer, warp 1 MMA, warps 2..5 epilogue
+constexpr int TC_THREADS = 288;    // warps 0..7 consumers (MMA + epilogue), warp 8 producer
 
 // operand packing: split into tf32 hi/lo and re-tile as [tile][kblk = KP/4][row group = R/8][8 rows][4 floats], the
-// UMMA canonical K-major no-swizzle layout, so that a K slab of a tile is one contiguous byte range
+// canonical K-major no-swizzle layout of wgmma, so that a K slab of a tile is one contiguous byte range
 template <int R>
 __device__ __forceinline__ void pack_split_one(int64_t t, int64_t n_rows, const int64_t* __restrict__ idx, const float* __restrict__ E,
                                                int64_t ld, int d, int KP, float* __restrict__ hi, float* __restrict__ lo) {

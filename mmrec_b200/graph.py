@@ -1,7 +1,7 @@
 """Graph builders feeding the propagation kernel: vectorised replacements of the reference's Python-dict /
 scipy builders.  Host logic (numpy) for the one-off normalised adjacency, device code for what changes per epoch.
 
-Reference code replaced (paths relative to /root/reference):
+Reference code replaced (paths relative to the root of enoche/MMRec):
   * `get_norm_adj_mat`  -- src/models/freedom.py:102-126 (copy-pasted in bm3/lightgcn/layergcn/encoders):
     a Python dict with 2E tuple keys, infeasible at 10^8 edges;
   * `MGCN.get_adj_mat`  -- src/models/mgcn.py:109-144 (lil-matrix slicing, 128 s at clothing scale);

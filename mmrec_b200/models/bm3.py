@@ -1,4 +1,4 @@
-"""BM3 on the B200 hot path; mirrors `/root/reference/src/models/bm3.py` (class name, config keys, parameter
+"""BM3 on the H100 hot path; mirrors `src/models/bm3.py` (class name, config keys, parameter
 names and order).  forward `:84-95` -> ops.propagate_mean; projections `:102-104` -> ops.project over the whole
 table (the dropout targets `:110-119` draw a mask over the whole projected table, so the gather cannot move in
 front of it without changing the RNG stream); full_sort_predict `:149-154` -> predictor + ops.score."""

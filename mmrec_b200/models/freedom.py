@@ -1,5 +1,5 @@
-"""FREEDOM on the B200 hot path.  Same class name, constructor, config keys, parameter names and registration
-order as `/root/reference/src/models/freedom.py` (so `init_seed` reproduces the same initial weights and a
+"""FREEDOM on the H100 hot path.  Same class name, constructor, config keys, parameter names and registration
+order as `src/models/freedom.py` (so `init_seed` reproduces the same initial weights and a
 reference `state_dict` loads), with the three op families delegated to `mmrec_b200.ops`:
 
   forward            `freedom.py:164-178`  -> ops.spmm / ops.propagate_mean (CSR SpMM, fused mean and `+ h`)

@@ -1,4 +1,4 @@
-"""LayerGCN on the B200 hot path; mirrors `/root/reference/src/models/layergcn.py` (the upstream file imports a
+"""LayerGCN on the H100 hot path; mirrors `src/models/layergcn.py` (the upstream file imports a
 non-existent `models.common`, `:12-13`; this one imports the real base).  forward `:125-138`: the cosine gate is
 fused into the SpMM epilogue for inference; training uses SpMM + torch ops so autograd sees the gate."""
 import random

@@ -1,4 +1,4 @@
-"""LightGCN on the B200 hot path; mirrors `/root/reference/src/models/lightgcn.py` (class name, config keys,
+"""LightGCN on the H100 hot path; mirrors `src/models/lightgcn.py` (class name, config keys,
 `embedding_dict` parameter names).  forward `:115-128` -> ops.propagate_mean; full_sort_predict `:156-164` -> ops.score."""
 import numpy as np
 import torch

@@ -1,4 +1,4 @@
-"""MGCN on the B200 hot path; mirrors `/root/reference/src/models/mgcn.py` (class name, config keys, parameter
+"""MGCN on the H100 hot path; mirrors `src/models/mgcn.py` (class name, config keys, parameter
 names and order).  Six SpMMs per forward (`:157-185`) -> ops.propagate_mean / ops.spmm on CSR; projections
 `:148-150` -> ops.project; the row-wise fusion (`:153-201`: purifier gates, 2-way attention, preference gates) is two
 kernels at inference (`ops.gate_rows`, `ops.mgcn_fuse`, SURVEY.md 8a a5b) and torch expressions under autograd."""

@@ -1,14 +1,11 @@
-"""MMGCN on the B200 hot path; mirrors `/root/reference/src/models/mmgcn.py` (class names, constructor, attribute and
+"""MMGCN on the H100 hot path; mirrors `src/models/mmgcn.py` (class names, constructor, attribute and
 parameter names, registration order) WITHOUT torch_geometric: PyG's `MessagePassing(aggr='mean')` with
 `message = x_j` (`mmgcn.py:191-213`) over the symmetrised edge list (`:40-42`) is the SpMM `D^-1 A (x W)`, run by
 `ops.spmm` on a row-normalised CSR; `MLP(features)` + `F.normalize` (`:165-168`) for the item rows is the fused
 gather -> linear -> L2-normalise kernel `ops.project(..., l2_normalize=True)`.
 
-Parity: torch_geometric is not installable in the build container; the reference's file was run under a shim of its one
-PyG primitive (tests/golden/ref_loader.py) to record tests/golden/mmgcn_tiny.npz.  This class reproduces that run --
-initial weights bit for bit, forward / loss / gradients / scores to fp32 rounding, the reference Trainer's metrics --
-under the reference's own harness with CPU stand-ins for the kernels (tests/test_dropin_contract.py), and the kernels are
-checked against `oracle.mmgcn_*` (pinned to the same file) in tests/test_gpu_models.py.  Unpinned: the mean aggregation
+Parity: torch_geometric is not a dependency; the reference's file was run under a shim of its one PyG primitive
+(tests/golden/ref_loader.py) to record tests/golden/mmgcn_tiny.npz, and the kernels are checked against `oracle.mmgcn_*` (pinned to the same file) in tests/test_gpu_models.py.  Unpinned: the mean aggregation
 primitive itself (shim and oracle restate PyG's documented formula).  Reference quirks kept on purpose: `concate = 'False'` is a non-empty string and
 therefore truthy, so the concatenating variant of every layer is the one that runs (`:31,129-137,171-172`);
 `preference`, `id_embedding` and `result` are plain tensors, not Parameters (`:55-56,127`), so the optimiser never

@@ -1,9 +1,9 @@
 """Host-side operators over the C ABI (include/mmrec_b200.h): the three op families of MMRec's hot path.
 
 Each function here replaces a PyTorch library call of the reference (cited per function, paths relative
-to /root/reference) with a call into libmmrec_b200.so on the current CUDA stream.  PyTorch is used for
+to the root of enoche/MMRec) with a call into libmmrec_b200.so on the current CUDA stream.  PyTorch is used for
 device memory, streams and autograd bookkeeping only.  There is no CPU path: tensors must live on a
-sm_100 device, otherwise `MMRecError` is raised.
+sm_90 device, otherwise `MMRecError` is raised.
 """
 from __future__ import annotations
 
@@ -18,9 +18,8 @@ _ws_cache: dict = {}
 import os as _os
 SEG = int(_os.environ.get("MMREC_SPMM_SEG", "512"))        # non-zeros per SpMM task (rows longer than this are split)
 LIGHT_MAX = int(_os.environ.get("MMREC_SPMM_LIGHT", "32"))  # tasks longer than this are run by a whole CTA
-# All SpMMs of an inference-time propagation in one cooperative launch (mmrec_spmm_chain_f32).  Measured on B200 at the baby
-# graph (profiles/r02_notes.md): 82.5 us against 75.8 us for one launch per SpMM replayed from a CUDA graph -- a grid-wide
-# barrier costs more than the launch boundary it replaces -- so it is opt-in.
+# All SpMMs of an inference-time propagation in one cooperative launch (mmrec_spmm_chain_f32).  Opt-in: a grid-wide barrier
+# per layer is not cheaper than the launch boundary it replaces when the launches are replayed from a CUDA graph.
 CHAIN = _os.environ.get("MMREC_SPMM_CHAIN", "0") == "1"
 
 
@@ -426,7 +425,7 @@ def project_raw(table, weight, bias, idx=None, l2_normalize=False) -> torch.Tens
 
 
 def set_project_path(tensor_core: bool):
-    """True (default): tcgen05 3xTF32 projection kernel; False: exact fp32 CUDA-core kernel."""
+    """True (default): wgmma 3xTF32 projection kernel; False: exact fp32 CUDA-core kernel."""
     _lib.load().mmrec_project_set_path(int(bool(tensor_core)))
 
 
@@ -580,8 +579,8 @@ def mgcn_fuse(img, txt, content, q_w, q_b, q_w2, gi_w, gi_b, gt_w, gt_b, want_si
 # K3: scoring, mask, top-k
 # ------------------------------------------------------------------------------------------------
 def set_score_path(path):
-    """"simt" (0): exact fp32 CUDA cores; "tc" (1): tcgen05 3xTF32 + mask + radix top-k kernels; "auto" (2, default):
-    fused where its shape rules allow, else tc; "fused" (3): tcgen05 with the top-k fused into the GEMM epilogue."""
+    """"simt" (0): exact fp32 CUDA cores; "tc" (1): wgmma 3xTF32 + mask + radix top-k kernels; "auto" (2, default):
+    fused where its shape rules allow, else tc; "fused" (3): wgmma f16 filter with the top-k fused into the GEMM epilogue."""
     if isinstance(path, str):
         path = {"simt": 0, "tc": 1, "auto": 2, "fused": 3}[path]
     _lib.load().mmrec_score_set_path(int(path))

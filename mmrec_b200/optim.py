@@ -1,7 +1,7 @@
 """f1: the optimiser step of the reference's trainer on the kernels of csrc/train.cu.
 
 `FusedAdam` is a drop-in for the `optim.Adam(params, lr=.., weight_decay=..)` the reference's trainer builds
-(`/root/reference/src/common/trainer.py:117-118`, stepped at `:189`): the same constructor arguments, `param_groups`, state
+(`src/common/trainer.py:117-118`, stepped at `:189`): the same constructor arguments, `param_groups`, state
 names (`step`, `exp_avg`, `exp_avg_sq`) and `state_dict` layout -- it IS a `torch.optim.Adam` whose `step` runs
 
 * `mmrec_adam_f32`: one launch for all ordinary parameters (torch's `_multi_tensor_adam` arithmetic), and
@@ -10,11 +10,9 @@ names (`step`, `exp_avg`, `exp_avg_sq`) and `state_dict` layout -- it IS a `torc
   `grad = G @ W`, and the kernel updates table, exp_avg and exp_avg_sq with that product computed on the fly -- the dense
   [n_items, F] gradient (115 MB per modality at Amazon-baby size) is never written or read.
 
-Measured on B200 (tools/bench_train.py, 7000 x 4096 table): the factored step takes 342 us (the CTA-per-column-strip
-access pattern moves the six table-sized streams at 2.0 TB/s), the dense route -- `mmrec_linear_dgrad_f32` writing the
-gradient, `mmrec_adam_f32` streaming everything linearly at 6.4 TB/s -- 120 + 124 us; torch/cuBLAS needs 101 + 490 us
-(profiles/r02_train.md).
-So `factored` is opt-in (`FusedAdam(..., factored=True)` or env MMREC_FACTORED_TABLE_GRAD=1): it trades time for not
+The factored step reads the table column strip by column strip, which streams HBM less efficiently than the dense route
+(`mmrec_linear_dgrad_f32` writing the gradient, then `mmrec_adam_f32` streaming everything linearly; compare with
+tools/bench_train.py).  So `factored` is opt-in (`FusedAdam(..., factored=True)` or env MMREC_FACTORED_TABLE_GRAD=1): it trades time for not
 holding the [n_items, F] gradient.  The factored form is only used where it is exact: a second backward before `step()` (gradient accumulation), a
 gradient from another path, `clip_grad_norm_` or a `weight` that changed since the backward make the pending product
 materialise into `.grad` (`materialize_pending`) and the table takes the ordinary route.  There is no CPU path.

@@ -76,9 +76,8 @@ class ItemShard:
 
     def csrs(self, device, d=64, l2_bytes=1 << 62):
         """(users x local items, local items x users) as device CSRs; a matrix whose dense operand ([n_cols, d] fp32) is
-        larger than `l2_bytes` comes as a column-panelled `ops.PanelCSR`.  (Off by default: measured on B200 the panels LOSE --
-        1.27 ms -> 2.19 ms per layer at 32M non-zeros, d = 64; 0.35 -> 0.67 ms at the xls shape -- because every panel
-        re-reads and re-writes the whole output for a handful of non-zeros per row; profiles/r02_notes.md.)"""
+        larger than `l2_bytes` comes as a column-panelled `ops.PanelCSR`.  (Off by default: every panel re-reads and
+        re-writes the whole output for a handful of non-zeros per row.)"""
         from .ops import CSR, PanelCSR
         u = torch.from_numpy(self.u).to(device)
         i = torch.from_numpy(self.i_local).to(device)

@@ -1,4 +1,4 @@
-"""Layered YAML configuration with the reference's semantics (`/root/reference/src/utils/configurator.py:46-129`):
+"""Layered YAML configuration with the reference's semantics (`src/utils/configurator.py:46-129`):
 overall.yaml < dataset/<name>.yaml < model/<Name>.yaml < config_dict; `hyper_parameters` lists accumulate;
 missing keys read as None.  YAML files live in `mmrec_b200/configs/` (override with `config_dir`) instead of
 `./configs` relative to the CWD."""

@@ -1,4 +1,4 @@
-"""Batch producers with the reference's output formats (`/root/reference/src/utils/dataloader.py`), vectorised.
+"""Batch producers with the reference's output formats (`src/utils/dataloader.py`), vectorised.
 
 * `TrainDataLoader` yields `LongTensor[3, B]` (user, positive, sampled negative) -- `[2, B]` when
   `use_neg_sampling` is False (`dataloader.py:226-260`).  The reference draws negatives one Python

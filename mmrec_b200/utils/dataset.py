@@ -1,4 +1,4 @@
-"""Interaction dataset with the reference's on-disk format and API (`/root/reference/src/utils/dataset.py:21-133`):
+"""Interaction dataset with the reference's on-disk format and API (`src/utils/dataset.py:21-133`):
 `<data_path>/<dataset>/<inter_file_name>` TSV with the user, item and `x_label` (0 train / 1 valid / 2 test) columns."""
 import os
 

@@ -1,4 +1,4 @@
-"""Run driver with the reference's flow (`/root/reference/src/utils/quick_start.py:19-108`): config -> dataset ->
+"""Run driver with the reference's flow (`src/utils/quick_start.py:19-108`): config -> dataset ->
 split -> dataloaders -> hyper-parameter grid (seed reset per combination) -> model + trainer -> summary."""
 import os
 import platform

@@ -1,9 +1,9 @@
 """Seeded synthetic Amazon-shaped interaction graphs (SURVEY.md Appendix C).
 
-There is no network on the build / GPU boxes, so every parity test and every
-bench number runs on graphs drawn here.  The on-disk layout written by
+Parity tests and bench numbers need no downloaded dataset: they run on graphs
+drawn here.  The on-disk layout written by
 :func:`write_dataset` is exactly what the reference reads
-(`/root/reference/src/utils/dataset.py:50-55` -- a TSV with the columns named in
+(`src/utils/dataset.py:50-55` -- a TSV with the columns named in
 `src/configs/dataset/baby.yaml:2-9` plus `x_label`; `image_feat.npy` /
 `text_feat.npy` per `baby.yaml:12-13`, loaded at
 `src/common/abstract_recommender.py:90-103`).

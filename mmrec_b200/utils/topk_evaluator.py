@@ -1,4 +1,4 @@
-"""Top-k evaluator with the reference's metric definitions (`/root/reference/src/utils/topk_evaluator.py:58-102`,
+"""Top-k evaluator with the reference's metric definitions (`src/utils/topk_evaluator.py:58-102`,
 `src/utils/metrics.py:12-105`): Recall / NDCG / Precision / MAP at each k of `config['topk']`, averaged over
 users, rounded to 4 decimals.  The hit matrix is built by a vectorised membership test instead of the reference's
 O(U * k * |pos|) Python loop (SURVEY.md 8f f2)."""

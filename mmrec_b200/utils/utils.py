@@ -1,4 +1,4 @@
-"""Small helpers with the reference's behaviour (`/root/reference/src/utils/utils.py:17-116`)."""
+"""Small helpers with the reference's behaviour (`src/utils/utils.py:17-116`)."""
 import datetime
 import importlib
 import random

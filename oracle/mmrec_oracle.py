@@ -4,7 +4,7 @@ A restatement, in plain numpy / torch-CPU fp32, of the algorithm on MMRec's hot
 path (SURVEY.md section 8a): graph normalisation, per-epoch edge pruning, LightGCN
 style sparse propagation, modality projection / fusion, full-catalog scoring and
 the trainer's mask + top-k.  Every function cites the reference lines it follows
-(paths relative to /root/reference).
+(paths relative to the root of enoche/MMRec).
 
 Who may import this file: `tests/`, `__graft_entry__.smoke()` and the
 `cpu_baseline` / `--impl reference` legs of `bench.py` -- as the checker or the
@@ -17,11 +17,11 @@ COO addmm, `mm`, `topk`.  The restatement therefore calls the same torch CPU ops
 in the same order, so on CPU it is bit-identical to the reference.
 
 PARITY PIN: the reference ships no tests / golden vectors (SURVEY.md section 4), so
-the oracle is pinned against outputs of the unmodified reference itself, run in the
-build container by `tests/golden/make_golden.py` and committed as
+the oracle is pinned against outputs of the unmodified reference itself, run by
+`tests/golden/make_golden.py` and committed as
 `tests/golden/*_tiny.npz`; `tests/test_oracle_golden.py` checks every function here
 against those files (bit-exact for indices and for values produced by the same
-torch ops).  MMGCN: torch_geometric is not installable here, so its one PyG primitive (`mmgcn_mean_aggregate`) stays
+torch ops).  MMGCN: torch_geometric is not a dependency, so its one PyG primitive (`mmgcn_mean_aggregate`) stays
 "parity unpinned"; the model code around it is pinned to the reference run under a shim of that primitive
 (tests/golden/mmgcn_tiny.npz).
 """

@@ -1,10 +1,12 @@
-"""Worker of tests/test_dropin_contract.py (own process: it imports the UNMODIFIED reference from /root/reference/src).
+"""Worker of tests/test_dropin_contract.py (own process: the kernels behind `mmrec_b200.ops` are patched).
 
-INTEGRATION.md section 2 claims that `mmrec_b200.models.FREEDOM` is a drop-in under the reference's own `quick_start` /
-`Trainer` / dataloaders.  This proves the claim without a GPU: the reference's Config, RecDataset, TrainDataLoader,
+INTEGRATION.md section 2 claims that the model classes of `mmrec_b200.models` are drop-ins under the reference's
+`quick_start` / `Trainer` / dataloaders.  This checks the claim without a GPU: a Config, RecDataset, TrainDataLoader,
 EvalDataLoader and Trainer are built exactly as `src/utils/quick_start.py:26-74` builds them, the model class is OURS, and the
 kernels behind `mmrec_b200.ops` are replaced by oracle-backed CPU stand-ins (test infrastructure: the product has no CPU
-path).  `Trainer.evaluate` (the reference's: full_sort_predict -> in-place mask -> torch.topk -> its own TopKEvaluator) must
+path).  The harness is the package's own restatement of the reference's (`mmrec_b200.utils`, `mmrec_b200.common.trainer`,
+taking the reference's dense evaluation route); with MMREC_REFERENCE_SRC set to the `src/` of an unmodified enoche/MMRec
+checkout it is the reference's own code.  Either way the results must equal the golden files recorded from the reference.  `Trainer.evaluate` (the reference's: full_sort_predict -> in-place mask -> torch.topk -> its own TopKEvaluator) must
 return the metrics recorded from the reference's own model, and one `calculate_loss` through `Trainer._train_epoch`'s call
 path must return the recorded loss."""
 import json
@@ -54,8 +56,9 @@ def install_cpu_ops():
     ops.project = lambda table, weight, bias=None, idx=None, l2_normalize=False: O.project(table, weight, bias, idx=idx, l2_normalize=l2_normalize)
     ops.score = lambda u, i, users=None: O.full_sort_scores(u, i, users if users is not None else torch.arange(u.shape[0]))
 
-    def mask_topk(scores, mask, k, item_offset=0):                    # graph._knn: selection of the kNN build
-        assert mask is None
+    def mask_topk(scores, mask, k, item_offset=0):                    # graph._knn, and the trainer's dense route
+        if mask is not None:
+            scores[mask[0], mask[1] - item_offset] = -1e10                # trainer.py:305-309
         return torch.topk(scores, k, dim=-1)
     ops.mask_topk = mask_topk
 
@@ -99,23 +102,40 @@ def install_cpu_ops():
     ops.propagate_layergcn = propagate_layergcn
 
 
+def harness(tmp):
+    """(data directory, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra config keys)."""
+    if os.environ.get("MMREC_REFERENCE_SRC"):
+        import ref_loader
+        ref_loader.install()
+        data = ref_loader.run_dir(tmp)
+        from utils.configurator import Config
+        from utils.dataset import RecDataset
+        from utils.dataloader import TrainDataLoader, EvalDataLoader
+        from utils.utils import init_seed
+        from common.trainer import Trainer
+        return data, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, {}
+    from mmrec_b200.common.trainer import Trainer
+    from mmrec_b200.utils.configurator import Config
+    from mmrec_b200.utils.dataloader import EvalDataLoader, TrainDataLoader
+    from mmrec_b200.utils.dataset import RecDataset
+    from mmrec_b200.utils.utils import init_seed
+    data = os.path.join(tmp, "data")
+    os.makedirs(data, exist_ok=True)
+    # the reference's routes: dense full_sort_predict -> mask -> top-k, host evaluator, torch.optim.Adam
+    extra = {"data_path": data + "/", "use_fused_topk": False, "device_evaluator": False, "fused_adam": False}
+    return data, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra
+
+
 def main():
-    import ref_loader
     from mmrec_b200.utils import synth
-    ref_loader.install()
     tmp = tempfile.mkdtemp(prefix="mmrec_contract_")
-    data = ref_loader.run_dir(tmp)
+    data, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra = harness(tmp)
     u, i, e, d, f = synth.SHAPES["tiny"]
     g = synth.make_graph(u, i, e, seed=0)
     v, t = synth.make_features(i, f, seed=1)
     synth.write_dataset(data, "tiny", g, v, t)
-    # --- the reference's own harness (src/utils/quick_start.py:26-74)
-    from utils.configurator import Config
-    from utils.dataset import RecDataset
-    from utils.dataloader import TrainDataLoader, EvalDataLoader
-    from utils.utils import init_seed
-    from common.trainer import Trainer
-    config = Config("FREEDOM", "tiny", {"gpu_id": 0, "use_gpu": False, "n_ui_layers": 3})
+    # --- the harness, built as src/utils/quick_start.py:26-74 builds it
+    config = Config("FREEDOM", "tiny", dict({"gpu_id": 0, "use_gpu": False, "n_ui_layers": 3}, **extra))
     config["inter_file_name"] = "tiny.inter"
     config["USER_ID_FIELD"], config["ITEM_ID_FIELD"] = "userID", "itemID"
     config["vision_feature_file"], config["text_feature_file"] = "image_feat.npy", "text_feat.npy"
@@ -159,23 +179,16 @@ def main():
 
 
 def main_mmgcn():
-    """The same for MMGCN: OUR class (no torch_geometric needed) under the reference's harness against
+    """The same for MMGCN: OUR class (no torch_geometric needed) under the harness against
     tests/golden/mmgcn_tiny.npz, the reference's own model code run under a PyG shim (tests/golden/ref_loader.py)."""
-    import ref_loader
     from mmrec_b200.utils import synth
-    ref_loader.install()
     tmp = tempfile.mkdtemp(prefix="mmrec_contract_")
-    data = ref_loader.run_dir(tmp)
+    data, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra = harness(tmp)
     u, i, e, d, f = synth.SHAPES["tiny"]
     g = synth.make_graph(u, i, e, seed=0)
     v, t = synth.make_features(i, f, seed=1)
     synth.write_dataset(data, "tiny", g, v, t)
-    from utils.configurator import Config
-    from utils.dataset import RecDataset
-    from utils.dataloader import TrainDataLoader, EvalDataLoader
-    from utils.utils import init_seed
-    from common.trainer import Trainer
-    config = Config("MMGCN", "tiny", {"gpu_id": 0, "use_gpu": False, "eval_batch_size": 128, "train_batch_size": 512})
+    config = Config("MMGCN", "tiny", dict({"gpu_id": 0, "use_gpu": False, "eval_batch_size": 128, "train_batch_size": 512}, **extra))
     config["inter_file_name"] = "tiny.inter"
     config["USER_ID_FIELD"], config["ITEM_ID_FIELD"] = "userID", "itemID"
     config["vision_feature_file"], config["text_feature_file"] = "image_feat.npy", "text_feat.npy"
@@ -221,25 +234,18 @@ def main_mmgcn():
 
 
 def main_model(name):
-    """BM3 / MGCN / LightGCN / LayerGCN: our class under the reference's harness against the golden file of the reference's
+    """BM3 / MGCN / LightGCN / LayerGCN: our class under the harness against the golden file of the reference's
     own class -- initial weights, `forward`, the loss on the recorded batch WITH the reference's RNG draws (BM3's always-on
     dropout: same `torch.manual_seed(4321)` stream as tests/golden/make_golden.py), first-batch scores, `Trainer.evaluate`."""
-    import ref_loader
     from mmrec_b200.utils import synth
-    ref_loader.install()
     tmp = tempfile.mkdtemp(prefix="mmrec_contract_")
-    data = ref_loader.run_dir(tmp)
+    data, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra = harness(tmp)
     u, i, e, d, f = synth.SHAPES["tiny"]
     g = synth.make_graph(u, i, e, seed=0)
     v, t = synth.make_features(i, f, seed=1)
     synth.write_dataset(data, "tiny", g, v, t)
-    from utils.configurator import Config
-    from utils.dataset import RecDataset
-    from utils.dataloader import TrainDataLoader, EvalDataLoader
-    from utils.utils import init_seed
-    from common.trainer import Trainer
     over = {"BM3": {}, "MGCN": {}, "LightGCN": {"n_layers": [3]}, "LayerGCN": {"dropout": [0.1]}}[name]
-    config = Config(name, "tiny", dict({"gpu_id": 0, "use_gpu": False, "eval_batch_size": 128, "train_batch_size": 512}, **over))
+    config = Config(name, "tiny", dict({"gpu_id": 0, "use_gpu": False, "eval_batch_size": 128, "train_batch_size": 512}, **over, **extra))
     config["inter_file_name"] = "tiny.inter"
     config["USER_ID_FIELD"], config["ITEM_ID_FIELD"] = "userID", "itemID"
     config["vision_feature_file"], config["text_feature_file"] = "image_feat.npy", "text_feat.npy"
@@ -304,32 +310,25 @@ def main_model(name):
     print("CONTRACT " + json.dumps(out))
 
 
-def main_traj(name):
-    """Two epochs of the reference's own training loop (`Trainer._train_epoch`, its Adam, its scheduler, its dataloader's
-    shuffling and negative sampling) driving OUR class, against the trajectory the reference's class produced
+def main_traj(key):
+    """Two epochs of the training loop (`Trainer._train_epoch`, its Adam, its scheduler, its dataloader's shuffling and
+    negative sampling) driving OUR class, against the trajectory the reference's class produced
     (tests/golden/traj_*_tiny.npz: every batch, every batch loss, per-epoch metrics)."""
-    import ref_loader
     from mmrec_b200.utils import synth
-    ref_loader.install()
     tmp = tempfile.mkdtemp(prefix="mmrec_contract_")
-    data = ref_loader.run_dir(tmp)
+    data, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra = harness(tmp)
     u, i, e, d, f = synth.SHAPES["tiny"]
     g = synth.make_graph(u, i, e, seed=0)
     v, t = synth.make_features(i, f, seed=1)
     synth.write_dataset(data, "tiny", g, v, t)
-    from utils.configurator import Config
-    from utils.dataset import RecDataset
-    from utils.dataloader import TrainDataLoader, EvalDataLoader
-    from utils.utils import init_seed
-    from common.trainer import Trainer
     # key -> (model class, overrides of make_golden.py's dump_trajectory call, golden file)
     name, over, gfile = {"LightGCN": ("LightGCN", {"n_layers": [2], "reg_weight": [1e-4]}, "traj_lightgcn_tiny.npz"),
                          "FREEDOM": ("FREEDOM", {"dropout": [0.0], "reg_weight": [1e-3]}, "traj_freedom_tiny.npz"),
                          "FREEDOM-prune": ("FREEDOM", {"dropout": [0.8], "reg_weight": [1e-3]}, "traj_freedom_prune_tiny.npz"),
                          "LayerGCN": ("LayerGCN", {"dropout": [0.1]}, "traj_layergcn_tiny.npz"),
                          "BM3": ("BM3", {}, "traj_bm3_tiny.npz"),
-                         "MGCN": ("MGCN", {}, "traj_mgcn_tiny.npz")}[name]
-    config = Config(name, "tiny", dict({"gpu_id": 0, "use_gpu": False, "eval_batch_size": 128, "train_batch_size": 512}, **over))
+                         "MGCN": ("MGCN", {}, "traj_mgcn_tiny.npz")}[key]
+    config = Config(name, "tiny", dict({"gpu_id": 0, "use_gpu": False, "eval_batch_size": 128, "train_batch_size": 512}, **over, **extra))
     config["inter_file_name"] = "tiny.inter"
     config["USER_ID_FIELD"], config["ITEM_ID_FIELD"] = "userID", "itemID"
     config["vision_feature_file"], config["text_feature_file"] = "image_feat.npy", "text_feat.npy"
@@ -360,14 +359,35 @@ def main_traj(name):
         rec["losses"].append(float(sum(l)) if isinstance(l, tuple) else float(l))
         return l
     model.calculate_loss = spy
+    # The reference's own loader reproduces its shuffling and negative-sampling stream, so its batches are compared.  The
+    # package's loader keeps the reference's batch format but draws its own stream (vectorised sampling), so with the
+    # package harness the recorded batches are replayed and every loss and metric is compared.
+    replay = not os.environ.get("MMREC_REFERENCE_SRC")
+    offs = np.concatenate([[0], np.cumsum(gold["batch_sizes"])])
+    first = np.concatenate([[0], np.cumsum(gold["batches_per_epoch"])])
+    recorded = [[torch.from_numpy(gold["batches"][:, offs[b]:offs[b + 1]]) for b in range(first[ep], first[ep + 1])]
+                for ep in range(len(gold["batches_per_epoch"]))]
+    # LayerGCN's uniform pruning draws from Python's `random`, the stream the reference's loader samples negatives from:
+    # its state at the start of each epoch is recorded from the reference run (MMREC_RECORD_DIR) and restored in replay.
+    import random
+    state_file = os.path.join(HERE, "golden", "traj_%s_tiny_pyrandom.npz" % key.lower())
+    states = []
     for ep in range(2):
+        if replay and os.path.isfile(state_file):
+            st = np.load(state_file)["state%d" % ep]
+            random.setstate((int(st[0]), tuple(int(x) for x in st[1:-1]), None))
+        states.append(np.array([random.getstate()[0]] + list(random.getstate()[1]) + [0], dtype=np.int64))
         model.pre_epoch_processing()
-        trainer._train_epoch(train_data, ep)
+        trainer._train_epoch(recorded[ep] if replay else train_data, ep)
         trainer.lr_scheduler.step()
         rec["valid"].append(list(trainer.evaluate(valid_data).values()))
         rec["test"].append(list(trainer.evaluate(test_data).values()))
+    if not replay and os.environ.get("MMREC_RECORD_DIR"):
+        np.savez(os.path.join(os.environ["MMREC_RECORD_DIR"], "traj_%s_tiny_pyrandom.npz" % key.lower()),
+                 **{"state%d" % ep: st for ep, st in enumerate(states)})
     batches = np.concatenate(rec["batches"], axis=1)
-    out = {"model": name, "same_batches": bool(batches.shape == gold["batches"].shape and np.array_equal(batches, gold["batches"])),
+    out = {"model": name, "batches": "recorded, replayed" if replay else "drawn by the reference's loader",
+           "same_batches": bool(batches.shape == gold["batches"].shape and np.array_equal(batches, gold["batches"])),
            "n_batches": len(rec["losses"]), "loss_max_rel": float(np.max(np.abs(np.array(rec["losses"]) - gold["losses"]) / np.abs(gold["losses"]))),
            "metric_max_abs": float(max(np.abs(np.array(rec["valid"]) - gold["valid"]).max(), np.abs(np.array(rec["test"]) - gold["test"]).max())),
            "first_loss": rec["losses"][0], "last_loss": rec["losses"][-1], "want_last_loss": float(gold["losses"][-1])}

@@ -1,9 +1,9 @@
 """Generate the golden vectors under tests/golden/ by RUNNING THE REFERENCE ITSELF.
 
-Run once in the build container (needs /root/reference; the GPU box only sees the
+Run once where an unmodified enoche/MMRec checkout is available (the tests only read the
 committed .npz files):
 
-    python tests/golden/make_golden.py
+    MMREC_REFERENCE_SRC=<MMRec checkout>/src python tests/golden/make_golden.py
 
 The reference has no tests, fixtures or known-answer vectors of its own
 (SURVEY.md section 4), so the pins are outputs of the unmodified reference code
@@ -288,7 +288,7 @@ def main():
     dump_mmgcn(common, os.path.join(HERE, "mmgcn_tiny.npz"))
     dump_trajectory("LightGCN", dict(common, n_layers=[2], reg_weight=[1e-4]), os.path.join(HERE, "traj_lightgcn_tiny.npz"))
     dump_trajectory("FREEDOM", dict(common, dropout=[0.0], reg_weight=[1e-3]), os.path.join(HERE, "traj_freedom_tiny.npz"))
-    # CPU contract trajectories (tests/test_dropin_contract.py): per-epoch pruning, dropout and the MGCN route in the loop
+    # CPU contract trajectories: per-epoch pruning, dropout and the MGCN route in the loop
     dump_trajectory("FREEDOM", dict(common, dropout=[0.8], reg_weight=[1e-3]), os.path.join(HERE, "traj_freedom_prune_tiny.npz"), slim=True)
     for fcache in os.listdir(os.path.join(data_root, DATASET)):
         if fcache.endswith(".pt"):

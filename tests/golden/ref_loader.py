@@ -1,7 +1,8 @@
-"""Import the UNMODIFIED reference (`/root/reference/src`) in this container.
+"""Import the UNMODIFIED reference (the `src/` directory of an enoche/MMRec checkout, named by the environment
+variable MMREC_REFERENCE_SRC).
 
-Only `tests/golden/make_golden.py` uses this, and only here (the GPU box has no
-`/root/reference`).  Nothing is copied: the reference is put on `sys.path` and
+Only `tests/golden/make_golden.py` and `tools/ref_vs_port_timing.py` use this; the tests read the committed
+golden files only.  Nothing is copied: the reference is put on `sys.path` and
 four import-time breakages of its environment pins (torch 1.11 / numpy 1.21 /
 scipy 1.7, `requirements.txt`) are shimmed, as listed in SURVEY.md Appendix A:
 
@@ -28,12 +29,12 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 
-REF_SRC = "/root/reference/src"
+REF_SRC = os.environ.get("MMREC_REFERENCE_SRC", "")             # src/ of an enoche/MMRec checkout
 
 
 def install():
     if not os.path.isdir(REF_SRC):
-        raise RuntimeError("reference tree not present (golden vectors are generated in the build container only)")
+        raise RuntimeError("set MMREC_REFERENCE_SRC to the src/ directory of an unmodified enoche/MMRec checkout")
     for name in ("lmdb", "matplotlib", "matplotlib.pyplot"):
         sys.modules.setdefault(name, types.ModuleType(name))
     ts = types.ModuleType("torch_scatter")

@@ -314,7 +314,7 @@ def test_fused_topk_operand_scaling(dev):
 
 
 def test_fused_topk_edge_cases(dev):
-    """The fused tcgen05 path (forced): heavy users (more masked items than there are item groups -> exact kernel),
+    """The fused tensor-core path (forced): heavy users (more masked items than there are item groups -> exact kernel),
     unsorted mask, degenerate (all-equal) scores, ragged sizes, d = 32 / 128."""
     from mmrec_b200 import ops
     ops.set_score_path("fused")

@@ -1,5 +1,5 @@
-"""Is `cpu_baseline.kind = "port"` a faithful stand-in for the reference's own speed?  Build container only (needs
-/root/reference): runs the UNMODIFIED reference FREEDOM (`src/models/freedom.py`, via tests/golden/ref_loader.py) and the
+"""Is `cpu_baseline.kind = "port"` a faithful stand-in for the reference's own speed?  Needs an unmodified enoche/MMRec
+checkout (MMREC_REFERENCE_SRC=<checkout>/src): runs the UNMODIFIED reference FREEDOM (`src/models/freedom.py`, via tests/golden/ref_loader.py) and the
 oracle port (`oracle/mmrec_oracle.py`, what `bench.py --impl reference` times) on the same baby-shaped synthetic dataset, same
 thread count, and prints the time of `forward` and of one `full_sort_predict` + mask + top-50 batch for both.
     python tools/ref_vs_port_timing.py [--threads 8]
