@@ -37,7 +37,7 @@ extern "C" {
 
 int mmrec_abi_version(void);
 const char* mmrec_last_error(void);
-/* 0 if the current device can run this library (compute capability 10.x), else MMREC_EUNSUPPORTED */
+/* 0 if the current device can run this library (compute capability 9.x), else MMREC_EUNSUPPORTED */
 int mmrec_device_check(void);
 /* Kernels of this library launched by the calling process so far (every launch site counts itself; library
  * primitives -- CUB sort/scan, memsets -- are not counted).  bench.py reports the difference over its timed region. */
@@ -229,6 +229,31 @@ int64_t mmrec_debug_fused_fallback_rows(const void* ws, int64_t B, int64_t n_ite
 /* tuning aid: with env MMREC_CF_TIMING set, device time in microseconds of the stages of the last fused call (host array
  * us[cap]; stages: catalogue pack | prep + mask | pass 1 | threshold | pass 2 | finalists | exact rows); returns the count */
 int mmrec_debug_cf_timing(float* us, int cap);
+
+/* K7  item-item cosine kNN of a feature table.   Replaces `sim = torch.mm(context_norm, context_norm.transpose(1, 0));
+ * torch.topk(sim, k, dim=-1)` of FREEDOM's `get_knn_adj_mat` (src/models/freedom.py:79-91) and of
+ * `build_knn_normalized_graph` (src/utils/utils.py:165-172); the caller passes the L2-normalised rows.
+ *
+ * mmrec_knn_topk_f32: for query rows j < m (table row rows[j]; rows == NULL means all rows, m == n), the top-k of
+ *                     X[rows[j]] . X[i] over all n rows i into out_idx / out_val [m, k]: values descending, equal values by
+ *                     ascending index -- the contract of mmrec_topk_rows_f32 -- and bit-identical to mmrec_score_f32 on
+ *                     its CUDA-core path followed by mmrec_topk_rows_f32, NaN included.  Tensor cores (fp16 operands,
+ *                     proven error bound, knn_cf.cu) only select candidates; every returned value is the exact fp32
+ *                     chain.  Rows the certificate cannot serve, and every row of a table holding a non-finite element,
+ *                     are computed by that exact route itself.  Synchronises `stream` (once per row block).
+ *                     Limits: n >= 1, 1 <= F, 1 <= k <= 1024, k <= n, n < 2^31, rows[j] in [0, n) (not checked);
+ *                     violations return MMREC_EINVAL, a workspace below mmrec_knn_topk_workspace_bytes(n, F, m, k)
+ *                     MMREC_EWORKSPACE.  m == 0 returns at once.
+ * mmrec_knn_topk_workspace_bytes: 0 for arguments outside those limits.  Holds the fp16 pack of X (2 n F bytes) plus
+ *                     bounded row-block scratch (<= ~1 GB).
+ * mmrec_debug_knn_fallback_rows: rows of the last mmrec_knn_topk_f32 call served by the exact route (all m when the table
+ *                     held a non-finite element), -1 before the first call.
+ * ------------------------------------------------------------------------------------------- */
+size_t mmrec_knn_topk_workspace_bytes(int64_t n, int F, int64_t m, int k);
+int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k,
+                       int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, void* stream);
+int64_t mmrec_debug_knn_fallback_rows(void);
+
 int mmrec_topk_merge(int parts, int64_t B, int k, const float* vals, const int64_t* idx,
                      int64_t* out_idx, float* out_val, void* stream);
 /* the same merge over lists left where each rank wrote them (peer-mapped memory): vals[p] / idx[p] are host

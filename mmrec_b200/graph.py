@@ -11,6 +11,8 @@ Reference code replaced (paths relative to the root of enoche/MMRec):
 """
 from __future__ import annotations
 
+from typing import Optional
+
 import numpy as np
 import torch
 
@@ -124,45 +126,70 @@ class EdgePruner:
 # ------------------------------------------------------------------------------------------------
 # item-item kNN graphs (init time)
 # ------------------------------------------------------------------------------------------------
-def _knn(feat: torch.Tensor, k: int):
+def _knn(feat: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None):
     """Cosine kNN of the item features (`sim = cn @ cn.T; torch.topk(sim, k)`, src/models/freedom.py:79-84,
-    src/utils/utils.py:165-172) on the scoring kernels (SURVEY.md 8f f4): the contraction is `ops.score` -- the same
-    `U I^T` as full_sort_predict with the normalised features on both sides (exact fp32 fmaf chains for F > 128) -- in row
-    blocks bounded to 256 MiB of similarities, the selection is `ops.mask_topk` (radix select, ties -> lower index)."""
+    src/utils/utils.py:165-172), for the query rows `rows` (default: all), ties -> lower index (SURVEY.md 8f f4).
+
+    F > 128 (every real feature table): `ops.knn_topk` (K7, csrc/knn_cf.cu) -- tensor-core candidate filter with the top-k
+    fused and every value an exact fp32 fmaf chain, bit-identical to the route below at these widths (where `ops.score`
+    is the exact CUDA-core kernel) without writing the [n, n] similarities.  F <= 128: `ops.score` (3xTF32 tensor-core
+    path) in row blocks bounded to 256 MiB of similarities, then `ops.mask_topk` (radix select)."""
     cn = feat.div(torch.norm(feat, p=2, dim=-1, keepdim=True)).contiguous()
+    if cn.shape[1] > 128:
+        return ops.knn_topk(cn, k, rows)
     n = cn.shape[0]
+    q = cn if rows is None else cn.index_select(0, rows.to(device=cn.device, dtype=torch.int64))
     vals, inds = [], []
     step = max(128, (256 << 20) // (4 * n))
-    for s in range(0, n, step):
-        sim = ops.score(cn[s:s + step], cn)
+    for s in range(0, q.shape[0], step):
+        sim = ops.score(q[s:s + step], cn)
         v, i = ops.mask_topk(sim, None, k)
         vals.append(v); inds.append(i)
     return torch.cat(vals), torch.cat(inds)
 
 
-def freedom_knn_coo(feat: torch.Tensor, k: int):
-    """`freedom.py:79-100`: directed cosine kNN, every edge weighs pow(k + 1e-7, -0.5)^2 in fp32."""
-    _, ind = _knn(feat, k)
+def freedom_knn_coo(feat: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None):
+    """`freedom.py:79-100`: directed cosine kNN, every edge weighs pow(k + 1e-7, -0.5)^2 in fp32.  `rows`: only the
+    edges leaving those items (row ids stay global).  Every item has exactly k out-edges, so the degree of every item is k
+    whichever rows are built: the rows are independent."""
+    _, ind = _knn(feat, k, rows)
     n = feat.shape[0]
-    row = torch.arange(n, device=feat.device).unsqueeze(1).expand(-1, k).reshape(-1)
+    src = torch.arange(n, device=feat.device) if rows is None else rows.to(device=feat.device, dtype=torch.int64)
+    row = src.unsqueeze(1).expand(-1, k).reshape(-1)
     col = ind.reshape(-1)
-    deg = torch.zeros(n, dtype=torch.int64, device=feat.device).index_add_(0, row, torch.ones_like(row))
+    if rows is None:
+        deg = torch.zeros(n, dtype=torch.int64, device=feat.device).index_add_(0, row, torch.ones_like(row))
+    else:
+        deg = torch.full((n,), k, dtype=torch.int64, device=feat.device)
     rinv = torch.pow(1e-7 + deg, -0.5)
     return row, col, rinv[row] * rinv[col]
 
 
-def build_freedom_mm_adj(v_feat, t_feat, k: int, image_weight: float) -> CSR:
-    """`freedom.py:67-75`: w * image_adj + (1 - w) * text_adj; shared edges add (CSR build sums duplicates)."""
+def freedom_mm_entries(v_feat, t_feat, k: int, image_weight: float, rows: Optional[torch.Tensor] = None):
+    """COO entries (pos, col, val) of `freedom.py:67-75`'s w * image_adj + (1 - w) * text_adj, image entries first, for
+    the rows `rows` (default: all): `pos` = j for an entry of row rows[j].  Shared edges are not yet summed."""
     parts = []
     if v_feat is not None:
-        parts.append((freedom_knn_coo(v_feat, k), image_weight if t_feat is not None else None))
+        parts.append((freedom_knn_coo(v_feat, k, rows), image_weight if t_feat is not None else None))
     if t_feat is not None:
-        parts.append((freedom_knn_coo(t_feat, k), (1.0 - image_weight) if v_feat is not None else None))
-    rows = torch.cat([p[0][0] for p in parts])
+        parts.append((freedom_knn_coo(t_feat, k, rows), (1.0 - image_weight) if v_feat is not None else None))
+    n = (v_feat if v_feat is not None else t_feat).shape[0]
+    if rows is None:
+        pos = torch.cat([p[0][0] for p in parts])
+    else:
+        own = torch.arange(rows.numel(), device=parts[0][0][0].device).unsqueeze(1).expand(-1, k).reshape(-1)
+        pos = torch.cat([own] * len(parts))
     cols = torch.cat([p[0][1] for p in parts])
     vals = torch.cat([p[0][2] if p[1] is None else p[1] * p[0][2] for p in parts])
-    n = (v_feat if v_feat is not None else t_feat).shape[0]
-    return CSR.from_coo(rows, cols, vals, n, n, sum_duplicates=True, symmetric=False)
+    return pos, cols, vals, n
+
+
+def build_freedom_mm_adj(v_feat, t_feat, k: int, image_weight: float, rows: Optional[torch.Tensor] = None) -> CSR:
+    """`freedom.py:67-75`: w * image_adj + (1 - w) * text_adj; shared edges add (CSR build sums duplicates).  `rows`: the
+    [len(rows), n] matrix whose row j is row rows[j] of mm_adj (FREEDOM's rows are independent, see freedom_knn_coo)."""
+    pos, cols, vals, n = freedom_mm_entries(v_feat, t_feat, k, image_weight, rows)
+    m = n if rows is None else rows.numel()
+    return CSR.from_coo(pos, cols, vals, m, n, sum_duplicates=True, symmetric=False)
 
 
 def build_mgcn_knn_adj(feat: torch.Tensor, k: int) -> CSR:

@@ -697,6 +697,45 @@ def fused_stage_times():
     return [float(buf[i]) for i in range(n)]
 
 
+def knn_topk(x: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None):
+    """Top-k of `x[rows] @ x.T` per query row (all rows by default) without the [m, n] similarity matrix
+    (`mmrec_knn_topk_f32`, K7): the cosine kNN of `src/models/freedom.py:79-91` / `src/utils/utils.py:165-172` for the
+    normalised feature table `x`.  Returns (values [m, k], indices int64 [m, k]), bit-identical to `score(x[rows], x)`
+    followed by `mask_topk(.., None, k)` on the CUDA-core path."""
+    _need_cuda(x, rows)
+    lib = _lib.load()
+    if x.dim() != 2:
+        raise MMRecError("knn_topk: x must be [n, F]")
+    x = _f32c(x)
+    n, F = x.shape
+    if rows is not None:
+        rows = rows.to(torch.int64).contiguous()
+        if rows.dim() != 1:
+            raise MMRecError("knn_topk: rows must be 1-D")
+        if rows.numel() and (int(rows.min()) < 0 or int(rows.max()) >= n):
+            raise MMRecError(f"knn_topk: rows outside [0, {n})")
+    m = n if rows is None else rows.numel()
+    if not (1 <= k <= min(1024, n)):
+        raise MMRecError(f"knn_topk: need 1 <= k <= min(1024, n = {n}), got {k}")
+    idx = torch.empty(m, k, dtype=torch.int64, device=x.device)
+    val = torch.empty(m, k, dtype=torch.float32, device=x.device)
+    if m == 0:
+        return val, idx
+    ws = _ws("knn", lib.mmrec_knn_topk_workspace_bytes(n, F, m, k) + 1024, x.device)
+    check(lib.mmrec_knn_topk_f32(n, _ptr(x), x.stride(0), F, m, _ptr(rows), k, _ptr(idx), _ptr(val), _ptr(ws), ws.numel(), _stream()),
+          "mmrec_knn_topk_f32")
+    # the graphs are built once, at model construction: the scratch (2 n F bytes of fp16 pack) is not kept for later calls
+    # (the call has synchronised the stream, so the memory is free to go back to the allocator)
+    _ws_cache.pop(("knn", x.device.index, torch.cuda.current_stream(x.device).cuda_stream), None)
+    return val, idx
+
+
+def knn_fallback_rows() -> int:
+    """Diagnostic: rows of the last `knn_topk` call that took the exact route (all of them when the table held a
+    non-finite element); -1 before the first call."""
+    return int(_lib.load().mmrec_debug_knn_fallback_rows())
+
+
 def topk_merge(vals: torch.Tensor, idx: torch.Tensor):
     """Merge per-shard top-k lists [parts, B, k] into the global top-k [B, k] (SURVEY.md 8e eval collective)."""
     _need_cuda(vals, idx)

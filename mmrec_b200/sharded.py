@@ -74,6 +74,24 @@ class ItemShard:
             return PanelCSR.from_coo(rt, ct, vt, self.n_local, n_cols, d, sum_duplicates=True)
         return CSR.from_coo(rt, ct, vt, self.n_local, n_cols, sum_duplicates=True)
 
+    def freedom_mm_csr(self, v_feat, t_feat, k, image_weight, device, d=64, l2_bytes=1 << 62):
+        """This rank's rows of FREEDOM's mm_adj built here from the full feature tables, no collective: the kNN of its own
+        items only (`graph.build_freedom_mm_adj(rows=...)`, rows are independent).  The same rank-major CSR `mm_csr` makes
+        from the global COO, bit for bit."""
+        from . import graph
+        from .ops import CSR, PanelCSR
+        if self.n_items % self.world:
+            raise ValueError("freedom_mm_csr: n_items must be a multiple of the world size (equal shards)")
+        mine = torch.from_numpy(self.local_items).to(device)
+        v = None if v_feat is None else v_feat.to(device)
+        t = None if t_feat is None else t_feat.to(device)
+        pos, col, val, _ = graph.freedom_mm_entries(v, t, k, image_weight, rows=mine)
+        col = (col % self.world) * self.n_local + col // self.world
+        n_cols = self.world * self.n_local
+        if n_cols * d * 4 > l2_bytes:
+            return PanelCSR.from_coo(pos, col, val, self.n_local, n_cols, d, sum_duplicates=True)
+        return CSR.from_coo(pos, col, val, self.n_local, n_cols, sum_duplicates=True)
+
     def csrs(self, device, d=64, l2_bytes=1 << 62):
         """(users x local items, local items x users) as device CSRs; a matrix whose dense operand ([n_cols, d] fp32) is
         larger than `l2_bytes` comes as a column-panelled `ops.PanelCSR`.  (Off by default: every panel re-reads and
