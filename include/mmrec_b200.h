@@ -254,6 +254,30 @@ int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F, int64_t m,
                        int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, void* stream);
 int64_t mmrec_debug_knn_fallback_rows(void);
 
+/* K8  full-table exp-sum of LGMRec's hypergraph contrastive loss.   Replaces `ttl_score = torch.exp(torch.matmul(norm_emb1,
+ * norm_all_emb.T) / self.tau).sum(dim=1)` of `ssl_triple_loss` (src/models/lgmrec.py:159-166) and its autograd, without the
+ * [B, M] matrix: wgmma 3xTF32, exp and the row sums in the accumulator registers (expsum.cu, which derives the error bound).
+ *
+ * mmrec_expsum_rows_f32:     ttl[b] = sum_{j < M} exp(<Q[b], T[j]> * inv_tau) for b < B.  Q [B, d] (row stride ldq), T [M, d]
+ *                            (ldt), fp32 row-major.  No maximum is subtracted: inf where the terms or their sum overflow.
+ *                            M == 0 gives ttl = 0; B == 0 returns at once.  Duplicate rows are allowed.
+ * mmrec_expsum_rows_bwd_f32: for the upstream gradient g [B]:  dQ[b] = g[b] * inv_tau * sum_j e_bj T[j],
+ *                            dT[j] = inv_tau * sum_b g[b] e_bj Q[b]  (e_bj recomputed, never stored).  dQ or dT may be NULL
+ *                            to skip it (not both).
+ *                            Both: d in {32, 64, 128}, B >= 0, M >= 0, leading dimensions >= d; violations and null pointers
+ *                            return MMREC_EINVAL, a workspace below mmrec_expsum_rows_workspace_bytes(B, M, d)
+ *                            MMREC_EWORKSPACE.  Results are bit-reproducible (fixed summation order, no atomics); the
+ *                            chunking depends on B and M only.
+ * mmrec_expsum_rows_workspace_bytes: for either call; O((B + M) d) (at most 32 partial slabs of B or 256 tile rows of M,
+ *                            0 when none is needed); 0 also for d outside {32, 64, 128} or negative sizes.
+ * ------------------------------------------------------------------------------------------- */
+size_t mmrec_expsum_rows_workspace_bytes(int64_t B, int64_t M, int d);
+int mmrec_expsum_rows_f32(int64_t B, const float* Q, int64_t ldq, int64_t M, const float* T, int64_t ldt, int d, float inv_tau,
+                          float* ttl, void* ws, size_t ws_bytes, void* stream);
+int mmrec_expsum_rows_bwd_f32(int64_t B, const float* Q, int64_t ldq, int64_t M, const float* T, int64_t ldt, int d, float inv_tau,
+                              const float* g, float* dQ, int64_t lddq, float* dT, int64_t lddt, void* ws, size_t ws_bytes,
+                              void* stream);
+
 int mmrec_topk_merge(int parts, int64_t B, int k, const float* vals, const int64_t* idx,
                      int64_t* out_idx, float* out_val, void* stream);
 /* the same merge over lists left where each rank wrote them (peer-mapped memory): vals[p] / idx[p] are host

@@ -736,6 +736,56 @@ def knn_fallback_rows() -> int:
     return int(_lib.load().mmrec_debug_knn_fallback_rows())
 
 
+# ------------------------------------------------------------------------------------------------
+# K8: full-table exp-sum (LGMRec's hypergraph contrastive loss)
+# ------------------------------------------------------------------------------------------------
+def _expsum_args(q, t):
+    _need_cuda(q, t)
+    if q.dim() != 2 or t.dim() != 2 or q.shape[1] != t.shape[1]:
+        raise MMRecError(f"expsum_rows: q {tuple(q.shape)} and t {tuple(t.shape)} must be [B, d] and [M, d]")
+    if q.shape[1] not in (32, 64, 128):
+        raise MMRecError(f"expsum_rows: d must be 32, 64 or 128, got {q.shape[1]}")
+    return _f32c(q), _f32c(t)
+
+
+class _ExpsumRowsFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, t, inv_tau: float):
+        q, t = _expsum_args(q, t)
+        ctx.save_for_backward(q, t)
+        ctx.inv_tau = inv_tau
+        lib = _lib.load()
+        (B, d), M = q.shape, t.shape[0]
+        ttl = torch.empty(B, dtype=torch.float32, device=q.device)
+        ws = _ws("expsum", lib.mmrec_expsum_rows_workspace_bytes(B, M, d), q.device)
+        check(lib.mmrec_expsum_rows_f32(B, _ptr(q), q.stride(0), M, _ptr(t), t.stride(0), d, inv_tau, _ptr(ttl), _ptr(ws), ws.numel(),
+                                        _stream()), "mmrec_expsum_rows_f32")
+        return ttl
+
+    @staticmethod
+    def backward(ctx, g):
+        q, t = ctx.saved_tensors
+        want_q, want_t = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (want_q or want_t):
+            return None, None, None
+        lib = _lib.load()
+        g = _f32c(g)
+        (B, d), M = q.shape, t.shape[0]
+        dq = torch.empty_like(q) if want_q else None
+        dt = torch.empty_like(t) if want_t else None
+        ws = _ws("expsum", lib.mmrec_expsum_rows_workspace_bytes(B, M, d), q.device)
+        check(lib.mmrec_expsum_rows_bwd_f32(B, _ptr(q), q.stride(0), M, _ptr(t), t.stride(0), d, ctx.inv_tau, _ptr(g), _ptr(dq), d,
+                                            _ptr(dt), d, _ptr(ws), ws.numel(), _stream()), "mmrec_expsum_rows_bwd_f32")
+        return dq, dt, None
+
+
+def expsum_rows(q: torch.Tensor, t: torch.Tensor, tau: float) -> torch.Tensor:
+    """`torch.exp(torch.matmul(q, t.T) / tau).sum(dim=1)` (`src/models/lgmrec.py:164`, the `ttl_score` of `ssl_triple_loss`)
+    without the [B, M] matrix, in the forward and in the backward (`mmrec_expsum_rows_f32` / `_bwd_f32`, K8), with
+    gradients for q and t.  d must be 32, 64 or 128."""
+    return _ExpsumRowsFn.apply(q, t, 1.0 / float(tau))
+
+
 def topk_merge(vals: torch.Tensor, idx: torch.Tensor):
     """Merge per-shard top-k lists [parts, B, k] into the global top-k [B, k] (SURVEY.md 8e eval collective)."""
     _need_cuda(vals, idx)
