@@ -281,27 +281,33 @@ __device__ __forceinline__ void cf_pack_one(int64_t t, int64_t n_rows, const int
         for (int e = 0; e < 8; ++e)
             if (kb * 8 + e < d) x[e] = __ldg(src + kb * 8 + e);
     }
-    float ss = 0.f;
     uint32_t am = 0u;                                                 // largest |x| as a bit pattern (orders like the value; NaN above inf)
+    if (!scale_src) {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { ss = fmaf(x[e], x[e], ss); const uint32_t b = __float_as_uint(x[e]) & 0x7fffffffu; am = b > am ? b : am; }
-    for (int o = kblks / 2; o > 0; o >>= 1) {
-        ss += __shfl_xor_sync(0xffffffffu, ss, o);
-        const uint32_t a2 = __shfl_xor_sync(0xffffffffu, am, o);
-        am = a2 > am ? a2 : am;
+        for (int e = 0; e < 8; ++e) { const uint32_t b = __float_as_uint(x[e]) & 0x7fffffffu; am = b > am ? b : am; }
+        for (int o = kblks / 2; o > 0; o >>= 1) {
+            const uint32_t a2 = __shfl_xor_sync(0xffffffffu, am, o);
+            am = a2 > am ? a2 : am;
+        }
     }
     const float sc = cf_scale_for(scale_src ? __ldg(scale_src) : am);
+    // the norm is taken of the scaled row: squares of unscaled elements below ~1e-19 underflow to 0 (and above ~1e19
+    // overflow), which would shrink the margin of cf_thr_kernel to its subnormal term while the operands are full size
+    float ss = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { x[e] *= sc; ss = fmaf(x[e], x[e], ss); }       // (exact: a power of two, no overflow)
+    for (int o = kblks / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
     uint32_t w[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-        const __half2 h = __floats2half2_rn(x[2 * e] * sc, x[2 * e + 1] * sc);
+        const __half2 h = __floats2half2_rn(x[2 * e], x[2 * e + 1]);
         w[e] = *reinterpret_cast<const uint32_t*>(&h);
     }
     const int64_t tile = row / CF_TILE;
     const int rr = (int)(row % CF_TILE);
     out[((tile * kblks + kb) * (CF_TILE / 8) + rr / 8) * 8 + (rr % 8)] = make_uint4(w[0], w[1], w[2], w[3]);
     if (kb == 0 && row < n_rows) {
-        const float nrm = sqrtf(ss) * sc * (1.0f + 1e-6f);            // norm of the scaled row (rounded up: the bound must hold)
+        const float nrm = sqrtf(ss) * (1.0f + 1e-6f);                 // norm of the scaled row (rounded up: the bound must hold)
         if (row_norm) row_norm[row] = nrm;
         if (max_norm) atomicMax(max_norm, __float_as_uint(nrm));      // non-negative floats order like their bit patterns
     }

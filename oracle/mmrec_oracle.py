@@ -451,6 +451,166 @@ def topk_tie_low_index(scores: np.ndarray, k: int):
 
 
 # --------------------------------------------------------------------------------------
+# the fused scorer's arithmetic, bit for bit (mmrec_b200/csrc/score_cf.cu, "exact fp32 score of one (user, item)
+# pair"): whichever of its kernels serves a row, the row is the top-k of these fp32 values under float_key
+# --------------------------------------------------------------------------------------
+
+MASKED_SCORE = np.float32(-1e10)                     # value of a masked item (src/common/trainer.py:307)
+_CANON_NAN = np.uint32(0x7FFFFFFF)                   # the NaN every CUDA fp32 instruction returns
+
+
+def _canon_nan(x: np.ndarray) -> np.ndarray:
+    x = np.array(x, dtype=np.float32, copy=True)
+    x.view(np.uint32)[np.isnan(x)] = _CANON_NAN
+    return x
+
+
+def fmaf32(a, b, c) -> np.ndarray:
+    """CUDA's `fmaf(a, b, c)` on fp32 arrays: a*b + c rounded once to nearest-even, subnormals kept, NaN canonical.
+
+    a*b is exact in float64 (24 + 24 significand bits, exponents in range); s = a*b + c is rounded in float64 and
+    TwoSum gives its exact error e.  Rounding s to float32 is then correct except when s sits exactly on a float32
+    midpoint with e != 0 (the true value is off the midpoint by e): that case takes the neighbour on the side of e."""
+    a, b, c = np.broadcast_arrays(np.asarray(a, np.float32), np.asarray(b, np.float32), np.asarray(c, np.float32))
+    with np.errstate(all="ignore"):
+        p = a.astype(np.float64) * b.astype(np.float64)
+        c64 = c.astype(np.float64)
+        s = p + c64
+        t = s - p
+        e = (p - (s - t)) + (c64 - t)
+        r = s.astype(np.float32)
+        fin = np.isfinite(s)
+        r64 = np.where(np.isinf(r) & fin, np.copysign(2.0 ** 128, s), r.astype(np.float64))   # overflow edge: 2^128
+        o = np.nextafter(r, np.where(s > r64, np.float32(np.inf), np.float32(-np.inf)).astype(np.float32))
+        mid = fin & (r64 != s) & ((r64 + o.astype(np.float64)) * 0.5 == s) & (e != 0)
+        out = np.where(mid, np.where(e > 0, np.maximum(r, o), np.minimum(r, o)), r)
+    return _canon_nan(out)
+
+
+def cf_lpr(d: int) -> int:
+    """Blocks of four elements in the chain: 8 / 16 / 32 for d <= 32 / 64 / 128."""
+    return 8 if d <= 32 else (16 if d <= 64 else 32)
+
+
+def cf_chain_scores(u, v) -> np.ndarray:
+    """fp32 scores of u [..., d] with v [..., d] (broadcast over the leading axes) in the fused scorer's arithmetic:
+    L = cf_lpr(d) blocks of four elements (zero beyond d), p_l = fmaf(u3,v3, fmaf(u2,v2, fmaf(u1,v1, fmaf(u0,v0, +0)))),
+    then p_a = p_a + p_(a+w) for a < w, w = L/2 .. 1; the score is p_0."""
+    u, v = np.asarray(u, np.float32), np.asarray(v, np.float32)
+    d = u.shape[-1]
+    assert v.shape[-1] == d and 1 <= d <= 128
+    L = cf_lpr(d)
+    shape = np.broadcast_shapes(u.shape[:-1], v.shape[:-1])
+    zero = np.zeros(shape, np.float32)
+    p = []
+    for blk in range(L):
+        acc = zero
+        for j in range(4 * blk, 4 * blk + 4):
+            # an element beyond d is fmaf(0, 0, acc) = acc + (+0): only a -0 changes (to +0)
+            acc = fmaf32(u[..., j], v[..., j], acc) if j < d else (acc + np.float32(0)).astype(np.float32)
+        p.append(acc)
+    w = L // 2
+    while w >= 1:
+        for a_ in range(w):
+            with np.errstate(all="ignore"):
+                p[a_] = (p[a_] + p[a_ + w]).astype(np.float32)
+        w //= 2
+    return _canon_nan(p[0])
+
+
+def float_key(x) -> np.ndarray:
+    """The kernels' order-preserving uint32 key (common.cuh): ascending key = ascending value, +0 > -0, +NaN largest."""
+    b = np.asarray(x, np.float32).view(np.uint32)
+    return np.where(b & np.uint32(0x80000000), ~b, b | np.uint32(0x80000000)).astype(np.uint32)
+
+
+def topk_float_key(vals, k: int, idx=None):
+    """Top-k of each row of `vals` [B, N] by float_key descending, then item index ascending (`idx` [B, N] or [N]:
+    the items' indices, default 0..N-1).  Returns (values fp32 [B, k], indices int64 [B, k])."""
+    vals = np.asarray(vals, np.float32)
+    if idx is None:
+        idx = np.arange(vals.shape[-1])
+    idx = np.broadcast_to(np.asarray(idx, np.int64), vals.shape)
+    order = np.lexsort((idx, np.uint32(0xFFFFFFFF) - float_key(vals)), axis=-1)[..., :k]
+    return np.take_along_axis(vals, order, -1), np.take_along_axis(idx, order, -1)
+
+
+def cf_exact_topk(user_e, item_e, users, mask, k: int, item_offset: int = 0, device=None, chunk_elems: int = 1 << 28):
+    """What `mmrec_score_topk` (fused path) must return, bit for bit: per row the top-k of the fp32 chain scores
+    (cf_chain_scores) with masked items at -1e10, by float_key then lower item index.  `mask` = [2, nnz] (batch row,
+    GLOBAL item column); entries outside [0, B) x [item_offset, item_offset + n_items) are ignored, duplicates allowed.
+
+    Emulating the chain over B x n_items is too slow on the host, so the fp64 scores s (torch, on `device`, in row chunks)
+    select the candidates first.  Per pair |chain - s| <= gamma = 16 * 2^-24 * |u| * max_i |v_i| (at most 9 roundings
+    on any path of the chain, Cauchy-Schwarz) + 192 * 2^-149 (underflow).  Hence the k-th largest chain value is
+    >= s_(k) - gamma and every member of the fp32 top-k has s >= s_(k) - 2 gamma: only those items are emulated.
+    Rows or catalogues holding a non-finite element are emulated over every item."""
+    dev = torch.device("cpu") if device is None else torch.device(device)
+    ue = torch.as_tensor(user_e).detach().to(dev, torch.float32)
+    ie = torch.as_tensor(item_e).detach().to(dev, torch.float32)
+    if users is not None:
+        ue = ue[torch.as_tensor(users).to(dev, torch.int64)]
+    B, d = ue.shape
+    n_items = ie.shape[0]
+    assert n_items >= k
+    u_np, i_np = ue.cpu().numpy(), ie.cpu().numpy()
+    # mask -> sorted unique (row, local item) pairs inside the batch and the shard
+    if mask is not None and torch.as_tensor(mask).numel() > 0:
+        m = torch.as_tensor(mask).cpu().to(torch.int64)
+        mr, mc = m[0], m[1] - item_offset
+        ok = (mr >= 0) & (mr < B) & (mc >= 0) & (mc < n_items)
+        key = torch.unique(mr[ok] * n_items + mc[ok])
+        mrow, mcol = (key // n_items).to(dev), (key % n_items).to(dev)
+    else:
+        mrow = mcol = torch.zeros(0, dtype=torch.int64, device=dev)
+    ie64 = ie.double()
+    vmax = ie64.norm(dim=1).max()
+    cat_finite = bool(torch.isfinite(ie).all())
+    row_finite = torch.isfinite(ue).all(dim=1).cpu().numpy()
+    out_v = np.empty((B, k), np.float32)
+    out_i = np.empty((B, k), np.int64)
+    full_rows = np.nonzero(~row_finite)[0].tolist() if cat_finite else list(range(B))
+    masked_val = float(MASKED_SCORE)
+    rows_per = max(1, chunk_elems // n_items)
+    pr, pi, extra = [], [], {}
+    for r0 in range(0, B if cat_finite else 0, rows_per):
+        r1 = min(B, r0 + rows_per)
+        u64 = ue[r0:r1].double()
+        s = u64 @ ie64.T
+        sel = (mrow >= r0) & (mrow < r1)
+        msk = torch.zeros_like(s, dtype=torch.bool)
+        msk[mrow[sel] - r0, mcol[sel]] = True
+        s = torch.where(msk, torch.full_like(s, masked_val), s)
+        gamma = 16 * 2.0 ** -24 * u64.norm(dim=1) * vmax + 192 * 2.0 ** -149
+        thr = torch.topk(s, k, dim=1).values[:, -1] - 2 * gamma
+        cand = (s >= thr[:, None]) & ~msk
+        rr, ii = torch.nonzero(cand, as_tuple=True)
+        pr.append(rr.cpu().numpy() + r0); pi.append(ii.cpu().numpy())
+        # masked items enter only when -1e10 itself is within reach; all equal, so the k lowest indices suffice
+        for r in torch.nonzero(thr <= masked_val).flatten().tolist():
+            extra[r0 + r] = torch.nonzero(msk[r]).flatten()[:k].cpu().numpy()
+    if cat_finite:
+        pr, pi = np.concatenate(pr), np.concatenate(pi)
+        keep = row_finite[pr]
+        pr, pi = pr[keep], pi[keep]
+        vals = cf_chain_scores(u_np[pr], i_np[pi])
+        starts = np.searchsorted(pr, np.arange(B + 1))          # nonzero() is row-major: pairs grouped by row
+        for r in np.nonzero(row_finite)[0]:
+            v, ix = vals[starts[r]:starts[r + 1]], pi[starts[r]:starts[r + 1]]
+            if r in extra:
+                v = np.concatenate([v, np.full(len(extra[r]), MASKED_SCORE)]); ix = np.concatenate([ix, extra[r]])
+            tv, ti = topk_float_key(v[None], k, ix[None])
+            out_v[r], out_i[r] = tv[0], ti[0]
+    mrow_np, mcol_np = mrow.cpu().numpy(), mcol.cpu().numpy()
+    for r in full_rows:                                         # every item: non-finite row or catalogue
+        v = cf_chain_scores(u_np[r][None, :], i_np)
+        v[mcol_np[mrow_np == r]] = MASKED_SCORE
+        tv, ti = topk_float_key(v[None], k)
+        out_v[r], out_i[r] = tv[0], ti[0]
+    return torch.from_numpy(out_v), torch.from_numpy(out_i + item_offset)
+
+
+# --------------------------------------------------------------------------------------
 # evaluator ("next" row f2; needed for Recall@20 parity) -- `src/utils/topk_evaluator.py:58-102`,
 # `src/utils/metrics.py:12-105`
 # --------------------------------------------------------------------------------------
