@@ -246,13 +246,15 @@ static AdamScalars adam_scalars(double beta1, double beta2, double eps, double w
     return AdamScalars{(float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, (float)weight_decay, (float)step_size, (float)bc2_sqrt};
 }
 
-// torch/optim/adam.py `_multi_tensor_adam` (the form torch.optim.Adam takes on CUDA tensors), one element:
-//   grad += weight_decay * param;  exp_avg.lerp_(grad, 1 - beta1);  exp_avg_sq = exp_avg_sq * beta2 + (1 - beta2) grad^2
-//   denom = sqrt(exp_avg_sq) / sqrt(1 - beta2^t) + eps;  param += -(lr / (1 - beta1^t)) * (exp_avg / denom)
+// torch/optim/adam.py `_multi_tensor_adam` (the form torch.optim.Adam takes on CUDA tensors), one element, with the
+// roundings of ATen's foreach kernels (oracle.adam_foreach_f32 restates them; tests/test_gpu_exact_arith.py compares bits):
+//   grad = fma(weight_decay, param, grad);  exp_avg = fma(1 - beta1, grad - exp_avg, exp_avg)        (_foreach_lerp_)
+//   exp_avg_sq = fma(1 - beta2, grad * grad, exp_avg_sq * beta2)   (_foreach_mul_, then _foreach_addcmul_: fma(value, t1 t2, x))
+//   denom = sqrt(exp_avg_sq) / sqrt(1 - beta2^t) + eps;  param = fma(-(lr / (1 - beta1^t)), exp_avg / denom, param)
 __device__ __forceinline__ void adam_update(float& p, float& m, float& v, float gr, const AdamScalars& a) {
     if (a.weight_decay != 0.f) gr = fmaf(a.weight_decay, p, gr);
     m = fmaf(a.w1, gr - m, m);
-    v = fmaf(a.w2 * gr, gr, v * a.beta2);
+    v = fmaf(a.w2, gr * gr, v * a.beta2);
     const float denom = sqrtf(v) / a.bc2_sqrt + a.eps;
     p = fmaf(a.step_size, m / denom, p);          // step_size = -lr / (1 - beta1^t): negative
 }

@@ -645,3 +645,160 @@ def topk_metrics(topk_index: np.ndarray, pos_items, topk=(5, 10, 20, 50), metric
         for k in topk:
             out[f"{m}@{k}"] = round(float(res[m][k - 1]), 4)                                  # topk_evaluator.py:99-101
     return out
+
+
+# --------------------------------------------------------------------------------------
+# exactly representable operands: inputs on which every correct kernel returns the exact result bit for bit
+# (tests/test_gpu_exact_arith.py).  Operands are integers times a power of two.  If every product is exact in fp32 and,
+# for each output, sum |a||b| < 2^22 in units of the product granularity, then every partial sum of every summation
+# order is an integer below 2^22 units, so an fp32 adder that keeps 24 bits after alignment never rounds: K splits,
+# chunk rotations, lane widths and tilings cannot change a bit.  Epilogues that round (a division, sqrt, a product)
+# are emulated below in numpy float32, whose +, -, *, / and sqrt are IEEE, correctly rounded.
+# --------------------------------------------------------------------------------------
+
+EXACT_BUDGET = 1 << 22                               # max sum |a||b| per output, in units of the product granularity
+
+
+def exact_ints(rng, shape, bits, density=1.0, signed=True, full=False):
+    """int64 array of `shape`: nonzero entries with at most `bits` significant bits (|m| < 2^bits), zeros elsewhere
+    with probability 1 - density.  `full`: every nonzero has EXACTLY `bits` significant bits (odd, >= 2^(bits-1)),
+    so a tf32 split of it into an 11-bit hi leaves a nonzero lo whenever bits > 11."""
+    if full and bits == 1:
+        m = np.ones(shape, dtype=np.int64)
+    elif full:
+        m = rng.integers(1 << (bits - 2), 1 << (bits - 1), size=shape, dtype=np.int64) * 2 + 1   # odd, in (2^(bits-1), 2^bits)
+    else:
+        m = rng.integers(0, 1 << bits, size=shape, dtype=np.int64)
+    if signed:
+        m = m * rng.choice(np.array([-1, 1], dtype=np.int64), size=shape)
+    if density < 1.0:
+        m = m * (rng.random(shape) < density)
+    return m
+
+
+def significant_bits(m) -> np.ndarray:
+    """Number of bits from the highest to the lowest set bit of |m| (0 for 0)."""
+    a = np.abs(np.asarray(m, dtype=np.int64))
+    out = np.zeros(a.shape, dtype=np.int64)
+    nz = a != 0
+    if nz.any():
+        v = a[nz]
+        low = (v & -v)
+        out[nz] = np.floor(np.log2(v.astype(np.float64))).astype(np.int64) - np.log2(low.astype(np.float64)).astype(np.int64) + 1
+    return out
+
+
+def to_f32_exact(m, scale: float) -> np.ndarray:
+    """m * scale as float32, asserting the conversion is exact (|m| < 2^24, scale a power of two)."""
+    m = np.asarray(m, dtype=np.int64)
+    assert np.frexp(scale)[0] == 0.5, "scale must be a power of two"
+    assert int(np.abs(m).max(initial=0)) < (1 << 24), "integer does not fit a float32 significand"
+    out = (m.astype(np.float64) * scale).astype(np.float32)
+    assert np.array_equal(out.astype(np.float64), m.astype(np.float64) * scale)
+    return out
+
+
+def int_matmul(a, b) -> np.ndarray:
+    """Exact a @ b of integer matrices through float64 BLAS (numpy's int64 matmul has no BLAS): exact while every
+    sum_k |a||b| is below 2^53, which is asserted."""
+    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+    assert float((np.abs(a) @ np.abs(b)).max(initial=0.0)) < 2.0 ** 53
+    return (a @ b).astype(np.int64)
+
+
+def exact_matmul_bound(a, b) -> int:
+    """max over outputs of sum_k |a[i,k]| |b[k,j]| for integer a [n, K] and b [K, m] (the precondition of exactness),
+    after asserting every single product is exact in fp32 (< 2^24)."""
+    a, b = np.abs(np.asarray(a, dtype=np.int64)), np.abs(np.asarray(b, dtype=np.int64))
+    assert int(a.max(initial=0)) * int(b.max(initial=0)) < (1 << 24), "a product is not exact in fp32"
+    return int(int_matmul(a, b).max(initial=0))
+
+
+def assert_exact_matmul(a, b, budget: int = EXACT_BUDGET) -> None:
+    s = exact_matmul_bound(a, b)
+    assert s < budget, f"exactness precondition broken: sum |a||b| = {s} >= {budget} units"
+
+
+def tf32_split_trunc(x):
+    """K2's split of the streamed table (`split_tf32_trunc`): hi = x with the low 13 mantissa bits cleared, lo = x - hi.
+    Returns (hi, lo, lo_tc): lo_tc is lo as the tensor core reads it (low 13 mantissa bits truncated)."""
+    x = np.asarray(x, dtype=np.float32)
+    hi = (x.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+    lo = (x - hi).astype(np.float32)
+    lo_tc = (lo.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+    return hi, lo, lo_tc
+
+
+def _tf32_rna(x):
+    """cvt.rna.tf32.f32: round to 10 mantissa bits, ties away from zero (finite inputs)."""
+    u = np.asarray(x, dtype=np.float32).view(np.uint32).astype(np.uint64)
+    r = ((u + np.uint64(0x1000)) & np.uint64(0xFFFFE000)).astype(np.uint32)
+    return r.view(np.float32)
+
+
+def tf32_split_rn(x):
+    """`split_tf32` (weights of K2, both operands of K3t): hi = rna_tf32(x), lo = rna_tf32(x - hi)."""
+    x = np.asarray(x, dtype=np.float32)
+    hi = _tf32_rna(x)
+    lo = _tf32_rna((x - hi).astype(np.float32))
+    return hi, lo
+
+
+def fdiv_f32(a, b) -> np.ndarray:
+    """`__fdiv_rn` / IEEE `/` in fp32."""
+    return (np.asarray(a, np.float32) / np.asarray(b, np.float32)).astype(np.float32)
+
+
+def spmm_epilogue_f32(y, acc_in=None, acc_div: float = 1.0, post=None, gate_ref=None, y_old=None):
+    """The fused SpMM epilogue of csrc/spmm.cu on an exact product y [n, d] (float32): optional LayerGCN gate
+    `y *= dot / (max(sqrt(ny), 1e-8) max(sqrt(nr), 1e-8))` (dot, ny, nr must be exact: the caller asserts it), then
+    Y = y (+ y_old), acc = ((y + acc_in) / acc_div) + post.  Returns (Y, acc)."""
+    f = np.float32
+    y = np.asarray(y, np.float32)
+    if gate_ref is not None:
+        r = np.asarray(gate_ref, np.float32)
+        dot = (y.astype(np.float64) * r).sum(1).astype(np.float32)
+        ny = (y.astype(np.float64) ** 2).sum(1).astype(np.float32)
+        nr = (r.astype(np.float64) ** 2).sum(1).astype(np.float32)
+        den = (np.maximum(np.sqrt(ny), f(1e-8)) * np.maximum(np.sqrt(nr), f(1e-8))).astype(np.float32)
+        c = (dot / den).astype(np.float32)
+        y = (y * c[:, None]).astype(np.float32)
+    Y = y if y_old is None else (np.asarray(y_old, np.float32) + y).astype(np.float32)
+    acc = y if acc_in is None else (y + np.asarray(acc_in, np.float32)).astype(np.float32)
+    if acc_div != 1.0:
+        acc = fdiv_f32(acc, f(acc_div))
+    if post is not None:
+        acc = (acc + np.asarray(post, np.float32)).astype(np.float32)
+    return Y, acc
+
+
+def l2_rows_f32(y) -> np.ndarray:
+    """K2's `y * (1 / max(sqrt(sum y^2), 1e-12))` per row (the sum must be exact: the caller asserts it)."""
+    y = np.asarray(y, np.float32)
+    ss = (y.astype(np.float64) ** 2).sum(1).astype(np.float32)
+    inv = (np.float32(1.0) / np.maximum(np.sqrt(ss), np.float32(1e-12))).astype(np.float32)
+    return (y * inv[:, None]).astype(np.float32)
+
+
+def adam_foreach_f32(p, g, m, v, step: int, lr: float, beta1: float, beta2: float, eps: float, weight_decay: float):
+    """One step of torch 2.11's `_multi_tensor_adam` (torch.optim.Adam(foreach=True) on CUDA, no amsgrad / maximize /
+    capturable) element by element in fp32: the ATen foreach kernels' operation order, with their FMAs.
+        grad = fma(wd, p, grad)                    _foreach_add(grads, params, alpha=wd)
+        m    = fma(1 - beta1, grad - m, m)         _foreach_lerp_(exp_avgs, grads, 1 - beta1)   (weight < 0.5 branch)
+        v    = v * beta2                           _foreach_mul_(exp_avg_sqs, beta2)
+        v    = fma(1 - beta2, grad * grad, v)      _foreach_addcmul_(..., value=1 - beta2)      (pointwise_op_impl)
+        den  = sqrt(v) / bc2_sqrt + eps            _foreach_sqrt, _foreach_div_, _foreach_add_
+        p    = fma(step_size, m / den, p)          _foreach_addcdiv_(params, exp_avgs, den, step_size)
+    Python-float scalars enter the kernels rounded to fp32.  Returns new (p, m, v)."""
+    f = np.float32
+    p, g, m, v = (np.asarray(x, np.float32) for x in (p, g, m, v))
+    if weight_decay != 0:
+        g = fmaf32(f(weight_decay), p, g)
+    m = fmaf32(f(1 - beta1), (g - m).astype(np.float32), m)
+    v = (v * f(beta2)).astype(np.float32)
+    v = fmaf32(f(1 - beta2), (g * g).astype(np.float32), v)
+    bc1, bc2 = 1 - beta1 ** step, 1 - beta2 ** step
+    step_size, bc2_sqrt = (lr / bc1) * -1, bc2 ** 0.5
+    den = ((np.sqrt(v) / f(bc2_sqrt)).astype(np.float32) + f(eps)).astype(np.float32)
+    p = fmaf32(f(step_size), (m / den).astype(np.float32), p)
+    return p, m, v
