@@ -553,7 +553,14 @@ def gate_rows(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor
     n, d = x.shape
     if weight.shape != (d, d):
         raise MMRecError(f"gate_rows: weight must be [{d}, {d}]")
-    out = torch.empty(n, d, dtype=torch.float32, device=x.device) if out is None else out
+    if bias is not None and bias.shape != (d,):
+        raise MMRecError(f"gate_rows: bias must be [{d}], got {tuple(bias.shape)}")
+    if mul is not None and mul.shape != (n, d):
+        raise MMRecError(f"gate_rows: mul must be [{n}, {d}], got {tuple(mul.shape)}")
+    if out is None:
+        out = torch.empty(n, d, dtype=torch.float32, device=x.device)
+    elif out.shape != (n, d) or out.dtype != torch.float32 or not out.is_contiguous() or out.device != x.device:
+        raise MMRecError(f"gate_rows: out must be a contiguous float32 [{n}, {d}] tensor on {x.device}")
     check(_lib.load().mmrec_gate_rows_f32(n, d, _ptr(x), _ptr(weight), _ptr(None if bias is None else _f32c(bias)),
                                           _ptr(None if mul is None else _f32c(mul)), _ptr(out), _stream()), "mmrec_gate_rows_f32")
     return out
@@ -567,6 +574,14 @@ def mgcn_fuse(img, txt, content, q_w, q_b, q_w2, gi_w, gi_b, gt_w, gt_b, want_si
     n, d = img.shape
     if txt.shape != (n, d) or content.shape != (n, d):
         raise MMRecError("mgcn_fuse: img, txt and content must share one shape")
+    for name, w in (("q_w", q_w), ("gi_w", gi_w), ("gt_w", gt_w)):
+        if w.shape != (d, d):
+            raise MMRecError(f"mgcn_fuse: {name} must be [{d}, {d}], got {tuple(w.shape)}")
+    for name, b in (("q_b", q_b), ("gi_b", gi_b), ("gt_b", gt_b)):
+        if b.shape != (d,):
+            raise MMRecError(f"mgcn_fuse: {name} must be [{d}], got {tuple(b.shape)}")
+    if q_w2.numel() != d:
+        raise MMRecError(f"mgcn_fuse: q_w2 must have {d} elements, got {q_w2.numel()}")
     out = torch.empty(n, d, dtype=torch.float32, device=img.device)
     side = torch.empty_like(out) if want_side else None
     check(_lib.load().mmrec_mgcn_fuse_f32(n, d, _ptr(img), _ptr(txt), _ptr(content), _ptr(_f32c(q_w)), _ptr(_f32c(q_b)),

@@ -802,3 +802,73 @@ def adam_foreach_f32(p, g, m, v, step: int, lr: float, beta1: float, beta2: floa
     den = ((np.sqrt(v) / f(bc2_sqrt)).astype(np.float32) + f(eps)).astype(np.float32)
     p = fmaf32(f(step_size), (m / den).astype(np.float32), p)
     return p, m, v
+
+
+def assert_bits(got, want, what: str = "") -> None:
+    """`got` equals `want` element for element (`torch.equal`; NaN matches NaN at the same position).  On failure the
+    message names how many elements differ and the first one.  Either side may be a tensor (any device) or an array."""
+    got = got.detach().cpu() if isinstance(got, torch.Tensor) else torch.from_numpy(np.asarray(got, np.float32))
+    want = want.detach().cpu() if isinstance(want, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(want, dtype=np.float32))
+    assert got.shape == want.shape, (what, got.shape, want.shape)
+    if got.is_floating_point() and want.is_floating_point():
+        nan_g, nan_w = torch.isnan(got), torch.isnan(want)
+        same = torch.equal(nan_g, nan_w) and torch.equal(got.masked_fill(nan_g, 0), want.masked_fill(nan_w, 0))
+    else:
+        same = torch.equal(got, want)
+    if not same:
+        bad = ((got != want) & ~(torch.isnan(got) & torch.isnan(want))) if got.is_floating_point() else (got != want)
+        i = tuple(bad.nonzero()[0].tolist())
+        raise AssertionError(f"{what}: {int(bad.sum())} of {got.numel()} elements differ; first at {i}: got {got[i].item()!r}, "
+                             f"want {want[i].item()!r}")
+
+
+# --------------------------------------------------------------------------------------
+# a5b (csrc/fuse.cu), K1c (csrc/csr.cu): the kernels' stated fp32 arithmetic, operation by operation
+# --------------------------------------------------------------------------------------
+
+def fuse_chain_f32(X, W, b=None) -> np.ndarray:
+    """The pre-activations of `gate_rows_kernel` / `mgcn_fuse_kernel`: acc[n, j] = b_j (+0 without a bias), then
+    acc = fmaf(W[j, k], X[n, k], acc) for k = 0 .. d-1, one correctly rounded fmaf each."""
+    X, W = np.asarray(X, np.float32), np.asarray(W, np.float32)
+    n, d = X.shape
+    assert W.shape == (d, d)
+    acc = np.zeros((n, d), np.float32) if b is None else np.broadcast_to(np.asarray(b, np.float32), (n, d)).copy()
+    for k in range(d):
+        acc = fmaf32(W[None, :, k], X[:, k, None], acc)
+    return acc
+
+
+def csr_coalesce_f32(row, col, val, n_rows: int, n_cols: int, sum_duplicates: bool = True):
+    """`mmrec_csr_from_coo`: a stable sort by key = row * n_cols + col, then (sum_duplicates) one entry per key whose
+    value is the sequential fp32 sum of its run in input order; `val` None counts 1.0 per entry.  Returns
+    (rowptr int64 [n_rows + 1], colidx int64 [nnz], vals float32 [nnz])."""
+    row, col = np.asarray(row, np.int64), np.asarray(col, np.int64)
+    val = np.ones(row.shape, np.float32) if val is None else np.asarray(val, np.float32)
+    key = row.astype(np.uint64) * np.uint64(n_cols) + col.astype(np.uint64)
+    order = np.argsort(key, kind="stable")
+    key, val = key[order], val[order]
+    if sum_duplicates and key.size:
+        head = np.flatnonzero(np.concatenate([[True], key[1:] != key[:-1]]))
+        ends = np.append(head[1:], key.size)
+        out = val[head].copy()
+        for r in range(1, int((ends - head).max())):      # r-th element of every run longer than r, added in order
+            live = head + r < ends
+            out[live] = (out[live] + val[head[live] + r]).astype(np.float32)
+        key, val = key[head], out
+    rows = (key // np.uint64(n_cols)).astype(np.int64)
+    rowptr = np.searchsorted(rows, np.arange(n_rows + 1), side="left").astype(np.int64)
+    return rowptr, (key % np.uint64(n_cols)).astype(np.int64), val.astype(np.float32)
+
+
+def bipartite_norm_f32(users, items, n_users: int, n_items: int, eps: float = 1e-7) -> np.ndarray:
+    """`mmrec_bipartite_norm_f32`: per edge fl(fl(1 / fl(sqrt(fl(float(deg_u) + eps)))) * the same for the item),
+    the degree converted to fp32 with round to nearest."""
+    users, items = np.asarray(users, np.int64), np.asarray(items, np.int64)
+    f, eps = np.float32, np.float32(eps)
+
+    def side(deg):
+        return (f(1.0) / np.sqrt((deg.astype(np.float32) + eps).astype(np.float32))).astype(np.float32)
+
+    ru = side(np.bincount(users, minlength=n_users))[users]
+    ri = side(np.bincount(items, minlength=n_items))[items]
+    return (ru * ri).astype(np.float32)

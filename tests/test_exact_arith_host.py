@@ -187,3 +187,86 @@ def test_adam_second_moment_forms_differ_by_one_ulp():
     later = float((O.fmaf32(w2, (g2 * g2).astype(np.float32), vb) != O.fmaf32((w2 * g2).astype(np.float32), g2, vb)).mean())
     assert 0.0 < later < first, later
     assert math.isfinite(first)
+
+
+def test_assert_bits_reports_the_first_difference_and_matches_nans():
+    a = np.array([[1.0, np.nan], [3.0, 4.0]], np.float32)
+    O.assert_bits(a, a.copy(), "same")
+    b = a.copy()
+    b[1, 0] = np.nextafter(np.float32(3.0), np.float32(4.0))
+    with pytest.raises(AssertionError, match=r"1 of 4 elements differ; first at \(1, 0\)"):
+        O.assert_bits(b, a, "one ulp")
+    c = a.copy()
+    c[0, 0] = np.nan
+    with pytest.raises(AssertionError, match="1 of 4"):
+        O.assert_bits(c, a, "NaN against a number")
+
+
+@pytest.mark.parametrize("with_bias", [True, False])
+def test_fuse_chain_is_a_sequential_fmaf_chain(with_bias):
+    """acc = b (or +0), then acc = fl(W[j, k] x_k + acc) for k = 0 .. d-1, each step one rounding of the exact value."""
+    rng = np.random.default_rng(6)
+    n, d = 5, 32
+    W = rng.standard_normal((d, d)).astype(np.float32)
+    X = (rng.standard_normal((n, d)) * np.exp2(rng.integers(-20, 20, (n, d)))).astype(np.float32)   # cancellation, mixed scales
+    X[1] = 0.0
+    b = rng.standard_normal(d).astype(np.float32) if with_bias else None
+    got = O.fuse_chain_f32(X, W, b)
+    for i in range(n):
+        for j in range(d):
+            acc = np.float32(0.0) if b is None else b[j]
+            for k in range(d):
+                acc = f32_round(F(W[j, k]) * F(X[i, k]) + F(acc))
+            assert got[i, j] == acc, (i, j)
+    assert np.array_equal(got[1], np.zeros(d, np.float32) if b is None else b)
+
+
+def test_csr_coalesce_sums_each_run_in_input_order():
+    """A stable sort by row * n_cols + col, then a sequential fp32 sum per key in input order; without summing, equal
+    keys keep their input order and their values."""
+    rng = np.random.default_rng(7)
+    n_rows, n_cols, nnz = 6, 5, 400
+    row, col = rng.integers(1, n_rows - 1, nnz), rng.integers(0, n_cols, nnz)      # rows 0 and 5 empty
+    val = (rng.standard_normal(nnz) * np.exp2(rng.integers(-12, 12, nnz))).astype(np.float32)
+    rowptr, colidx, vals = O.csr_coalesce_f32(row, col, val, n_rows, n_cols)
+    order = sorted(range(nnz), key=lambda i: (row[i], col[i]))                      # Python's sort is stable
+    keys, sums = [], []
+    for i in order:
+        if keys and keys[-1] == (row[i], col[i]):
+            sums[-1] = np.float32(sums[-1] + val[i])
+        else:
+            keys.append((row[i], col[i]))
+            sums.append(val[i])
+    assert colidx.tolist() == [c for _, c in keys] and np.array_equal(vals, np.array(sums, np.float32))
+    assert rowptr.tolist() == [sum(1 for r, _ in keys if r < q) for q in range(n_rows + 1)]
+    backwards = [np.float32(0)] * len(keys)                                          # the order is visible in the bits
+    for i in reversed(order):
+        k = keys.index((row[i], col[i]))
+        backwards[k] = np.float32(backwards[k] + val[i])
+    assert not np.array_equal(vals, np.array(backwards, np.float32))
+    _, c1, v1 = O.csr_coalesce_f32(row, col, None, n_rows, n_cols)                   # no values: each entry counts 1
+    assert np.array_equal(v1, np.array([sum(1 for i in order if (row[i], col[i]) == kk) for kk in keys], np.float32))
+    rp, c2, v2 = O.csr_coalesce_f32(row, col, val, n_rows, n_cols, sum_duplicates=False)
+    assert c2.tolist() == [col[i] for i in order] and np.array_equal(v2, val[order]) and rp[-1] == nnz
+    rp, c0, v0 = O.csr_coalesce_f32(np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, np.float32), 3, 4)
+    assert rp.tolist() == [0, 0, 0, 0] and c0.size == 0 and v0.size == 0
+
+
+def test_bipartite_norm_is_four_ieee_operations_per_side():
+    eps = 1e-7
+    users = np.array([0, 0, 1, 3, 3, 3], np.int64)
+    items = np.array([1, 0, 1, 1, 2, 1], np.int64)
+    got = O.bipartite_norm_f32(users, items, 5, 4, eps)
+
+    def side(deg):
+        x = f32_round(F(np.float32(deg)) + F(np.float32(eps)))
+        s = np.sqrt(np.float32(x))
+        assert _sqrt_f32_ok(np.float32(x), s)
+        return f32_round(Fraction(1) / F(s))
+
+    du, di = np.bincount(users, minlength=5), np.bincount(items, minlength=4)
+    for e in range(users.size):
+        assert got[e] == f32_round(F(side(du[users[e]])) * F(side(di[items[e]]))), e
+    # the degree's int -> float conversion rounds to nearest even above 2^24
+    big = O.bipartite_norm_f32(np.zeros((1 << 24) + 3, np.int64), np.arange((1 << 24) + 3) % 3, 1, 3)
+    assert big[0] == f32_round(F(side((1 << 24) + 4)) * F(side(-(-((1 << 24) + 3) // 3))))          # item 0: ceil(n / 3) edges

@@ -42,16 +42,6 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _assert_bits(got, want, what=""):
-    got = got.detach().cpu() if isinstance(got, torch.Tensor) else torch.from_numpy(np.asarray(got, np.float32))
-    want = torch.from_numpy(np.ascontiguousarray(want, dtype=np.float32)) if not isinstance(want, torch.Tensor) else want.detach().cpu()
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    if not torch.equal(got, want):
-        bad = (got != want).nonzero()
-        i = tuple(bad[0].tolist())
-        pytest.fail(f"{what}: {bad.shape[0]} of {got.numel()} elements differ; first at {i}: got {float(got[i])!r}, want {float(want[i])!r}")
-
-
 # ======================================================================================================================
 # K1: SpMM
 # ======================================================================================================================
@@ -122,7 +112,7 @@ def _run_epilogues(dev, case, use_plan, what):
     n = case.n
     Y = torch.full((n, d), 7.0, device=dev)
     ops.spmm_raw(case.A, case.X, Y=Y, use_plan=use_plan)
-    _assert_bits(Y, case.y, f"{what} Y")
+    O.assert_bits(Y, case.y, f"{what} Y")
     acc_in = torch.from_numpy(case.acc_in).to(dev)
     post = torch.from_numpy(case.post).to(dev)
     for div in (1.0, 4.0, 3.0):
@@ -130,25 +120,25 @@ def _run_epilogues(dev, case, use_plan, what):
         Y2 = torch.empty(n, d, device=dev)
         ops.spmm_raw(case.A, case.X, Y=Y2, acc_in=acc_in, acc_out=out, acc_div=div, use_plan=use_plan)
         _, want = O.spmm_epilogue_f32(case.y, case.acc_in, div)
-        _assert_bits(out, want, f"{what} acc_out (acc_div {div})")
-        _assert_bits(Y2, case.y, f"{what} Y beside acc_out")
+        O.assert_bits(out, want, f"{what} acc_out (acc_div {div})")
+        O.assert_bits(Y2, case.y, f"{what} Y beside acc_out")
     out = torch.empty(n, d, device=dev)                              # acc_out without acc_in, divided
     ops.spmm_raw(case.A, case.X, acc_out=out, acc_div=3.0, use_plan=use_plan)
-    _assert_bits(out, O.spmm_epilogue_f32(case.y, None, 3.0)[1], f"{what} acc_out / 3 without acc_in")
+    O.assert_bits(out, O.spmm_epilogue_f32(case.y, None, 3.0)[1], f"{what} acc_out / 3 without acc_in")
     # LayerGCN's gate on Y and on the running sum
     ref = torch.from_numpy(case.ref).to(dev)
     Yg, accg = torch.empty(n, d, device=dev), torch.empty(n, d, device=dev)
     ops.spmm_raw(case.A, case.X, Y=Yg, acc_in=acc_in, acc_out=accg, gate_ref=ref, use_plan=use_plan)
     wy, wa = O.spmm_epilogue_f32(case.y, case.acc_in, 1.0, gate_ref=case.ref)
-    _assert_bits(Yg, wy, f"{what} gated Y")
-    _assert_bits(accg, wa, f"{what} gated acc_out")
+    O.assert_bits(Yg, wy, f"{what} gated Y")
+    O.assert_bits(accg, wa, f"{what} gated acc_out")
     # Y += A X (mmrec_spmm_acc_f32) with a running sum
     Ya = torch.from_numpy(case.acc_in).to(dev).clone()
     outa = torch.empty(n, d, device=dev)
     ops.spmm_raw(case.A, case.X, Y=Ya, acc_in=acc_in, acc_out=outa, acc_div=3.0, use_plan=use_plan, y_accumulate=True)
     wy, wa = O.spmm_epilogue_f32(case.y, case.acc_in, 3.0, y_old=case.acc_in)
-    _assert_bits(Ya, wy, f"{what} Y += AX")
-    _assert_bits(outa, wa, f"{what} acc_out of the accumulating form")
+    O.assert_bits(Ya, wy, f"{what} Y += AX")
+    O.assert_bits(outa, wa, f"{what} acc_out of the accumulating form")
 
 
 def _lane_widths(d):
@@ -210,8 +200,8 @@ def test_spmm_misaligned_and_strided_through_the_c_abi(dev, d, shift):
     _, Rv = strided(case.ref, ldg, shift)
     _spmm_abi(case, d, Xv.data_ptr(), ldx, Yv.data_ptr(), ldy, Iv.data_ptr(), Ov.data_ptr(), ldacc, 3.0, Rv.data_ptr(), ldg)
     wy, wa = O.spmm_epilogue_f32(case.y, case.acc_in, 3.0, gate_ref=case.ref)
-    _assert_bits(Yv[:, :d], wy, "strided gated Y")
-    _assert_bits(Ov[:, :d], wa, "strided gated acc_out / 3")
+    O.assert_bits(Yv[:, :d], wy, "strided gated Y")
+    O.assert_bits(Ov[:, :d], wa, "strided gated acc_out / 3")
     assert bool((Yv[:, d:] == 5.0).all()) and bool((Ov[:, d:] == 5.0).all()), "wrote past d"
 
 
@@ -226,7 +216,7 @@ def test_spmm_transpose(dev, d):
     At = case.A.t()
     out = torch.empty(N_COLS, d, device=dev)
     ops.spmm_raw(At, torch.from_numpy(O.to_f32_exact(Gi, X_SCALE)).to(dev), Y=out)
-    _assert_bits(out, want, "A^T G")
+    O.assert_bits(out, want, "A^T G")
 
 
 @pytest.mark.parametrize("d", [64, 128])
@@ -241,8 +231,8 @@ def test_spmm_panel_csr(dev, d):
     Y, out = torch.empty(case.n, d, device=dev), torch.empty(case.n, d, device=dev)
     ops.spmm_raw(P, case.X, Y=Y, acc_in=torch.from_numpy(case.acc_in).to(dev), acc_out=out, acc_div=3.0)
     wy, wa = O.spmm_epilogue_f32(case.y, case.acc_in, 3.0)
-    _assert_bits(Y, wy, "panelled Y")
-    _assert_bits(out, wa, "panelled acc_out / 3")
+    O.assert_bits(Y, wy, "panelled Y")
+    O.assert_bits(out, wa, "panelled acc_out / 3")
 
 
 @pytest.mark.parametrize("d", [32, 64, 256])
@@ -281,7 +271,7 @@ def test_spmm_chain_with_post_rows(dev, d):
     before = ops.launch_count()
     got = ops.propagate_mean_fused(A, ego, 2, post_csr=M, post_x=torch.from_numpy(O.to_f32_exact(xi, 1.0)).to(dev), post_row0=row0)
     assert ops.launch_count() - before == 1, "the chained kernel did not take this shape"
-    _assert_bits(got, want, "chained mean + post")
+    O.assert_bits(got, want, "chained mean + post")
 
 
 # ======================================================================================================================
@@ -366,9 +356,9 @@ def test_project_tc_exact(dev, n_out, F, d, splits, low_on):
     bias = torch.from_numpy(O.to_f32_exact(b, ts * ws)).to(dev)
     ops.set_project_path(True)
     got = ops.project_raw(table, W, bias, torch.from_numpy(idx).to(dev))
-    _assert_bits(got, O.to_f32_exact(with_b, ts * ws), f"gathered + bias ({low_on} carries the low bits)")
+    O.assert_bits(got, O.to_f32_exact(with_b, ts * ws), f"gathered + bias ({low_on} carries the low bits)")
     got = ops.project_raw(table[:n_out], W, None)
-    _assert_bits(got, O.to_f32_exact(O.int_matmul(T[:n_out], Wt.T), ts * ws), f"whole table, no bias ({low_on} carries the low bits)")
+    O.assert_bits(got, O.to_f32_exact(O.int_matmul(T[:n_out], Wt.T), ts * ws), f"whole table, no bias ({low_on} carries the low bits)")
 
 
 @pytest.mark.parametrize("path", ["tc", "simt"])
@@ -394,9 +384,9 @@ def test_project_l2_normalize_and_misaligned_table(dev, n_out, F, d, path):
     ops.set_project_path(path == "tc")
     try:
         got = ops.project_raw(table, W, torch.from_numpy(O.to_f32_exact(b, 1.0)).to(dev), l2_normalize=True)
-        _assert_bits(got, O.l2_rows_f32(O.to_f32_exact(Yb, 1.0)), f"{path}: l2-normalised rows")
+        O.assert_bits(got, O.l2_rows_f32(O.to_f32_exact(Yb, 1.0)), f"{path}: l2-normalised rows")
         got = ops.project_raw(table, W, None)
-        _assert_bits(got, O.to_f32_exact(Y, 1.0), f"{path}: misaligned table")
+        O.assert_bits(got, O.to_f32_exact(Y, 1.0), f"{path}: misaligned table")
     finally:
         ops.set_project_path(True)
 
@@ -424,7 +414,7 @@ def test_score_exact(dev, B, I, d, low_on, path):
         got = ops.score(ue, ie, torch.from_numpy(users).to(dev))
     finally:
         ops.set_score_path("auto")
-    _assert_bits(got, want, f"{path} scores ({low_on} carries the low bits)")
+    O.assert_bits(got, want, f"{path} scores ({low_on} carries the low bits)")
 
 
 @pytest.mark.parametrize("path", ["tc", "simt"])
@@ -445,9 +435,9 @@ def test_score_mask_topk_on_integer_scores(dev, B, I, d, k, path):
         S = ops.score(torch.from_numpy(O.to_f32_exact(Ui, 1.0)).to(dev), torch.from_numpy(O.to_f32_exact(Ii, 1.0)).to(dev))
     finally:
         ops.set_score_path("auto")
-    _assert_bits(S, s, f"{path} integer scores")
+    O.assert_bits(S, s, f"{path} integer scores")
     val, idx = ops.mask_topk(S, torch.from_numpy(mask).to(dev), k)
-    _assert_bits(val, wv, "top-k values")
+    O.assert_bits(val, wv, "top-k values")
     assert np.array_equal(idx.cpu().numpy(), wi), "top-k indices (ties towards the lower index)"
 
 
@@ -509,7 +499,7 @@ def test_index_sum_rows_exact(dev, n_idx, n_rows, d):
     cnt = np.bincount(idx, minlength=n_rows) if n_idx else np.zeros(n_rows, np.int64)
     assert int(cnt.max(initial=0)) * 63 < O.EXACT_BUDGET
     got = ops.index_sum_rows(torch.from_numpy(O.to_f32_exact(g, 2.0 ** -5)).reshape(n_idx, d).to(dev), torch.from_numpy(idx).to(dev), n_rows)
-    _assert_bits(got, O.to_f32_exact(want, 2.0 ** -5), "index_sum_rows")
+    O.assert_bits(got, O.to_f32_exact(want, 2.0 ** -5), "index_sum_rows")
 
 
 @pytest.mark.parametrize("n,n_table,F,d,gather,bias", [
@@ -532,9 +522,9 @@ def test_linear_wgrad_exact(dev, n, n_table, F, d, gather, bias):
     O.assert_exact_matmul(up.T, x)
     dW, db = ops.linear_wgrad(torch.from_numpy(O.to_f32_exact(up, 2.0 ** -4)).to(dev), torch.from_numpy(O.to_f32_exact(T, 0.5)).to(dev),
                               None if idx is None else torch.from_numpy(idx).to(dev), want_bias=bias)
-    _assert_bits(dW, O.to_f32_exact(O.int_matmul(up.T, x), 2.0 ** -5), "dW")
+    O.assert_bits(dW, O.to_f32_exact(O.int_matmul(up.T, x), 2.0 ** -5), "dW")
     if bias:
-        _assert_bits(db, O.to_f32_exact(up.sum(0), 2.0 ** -4), "db")
+        O.assert_bits(db, O.to_f32_exact(up.sum(0), 2.0 ** -4), "db")
 
 
 # DgradShape<64, 512> (d <= 64) and <128, 256> (d > 64, k chunks of 128 accumulated by the store form); STORE (aligned,
@@ -548,7 +538,7 @@ def test_linear_dgrad_exact(dev, n_rows, F, d):
     W = O.exact_ints(rng, (d, F), 4)
     O.assert_exact_matmul(G, W)
     got = ops.linear_dgrad(torch.from_numpy(O.to_f32_exact(G, 2.0 ** -8)).to(dev), torch.from_numpy(O.to_f32_exact(W, 2.0 ** -2)).to(dev))
-    _assert_bits(got, O.to_f32_exact(O.int_matmul(G, W), 2.0 ** -10), "G @ W")
+    O.assert_bits(got, O.to_f32_exact(O.int_matmul(G, W), 2.0 ** -10), "G @ W")
 
 
 # ======================================================================================================================
@@ -578,10 +568,10 @@ def _assert_adam(got, want, what):
     (p, m, v), (wp, wm, wv) = ((x.detach().cpu() if isinstance(x, torch.Tensor) else torch.from_numpy(np.asarray(x, np.float32))
                                 for x in t) for t in (got, want))
     diff = float((v != wv).double().mean())
-    _assert_bits(m, wm, f"{what}: exp_avg")
+    O.assert_bits(m, wm, f"{what}: exp_avg")
     assert diff == 0.0, f"{what}: {100 * diff:.2f} % of exp_avg_sq elements differ"
-    _assert_bits(v, wv, f"{what}: exp_avg_sq")
-    _assert_bits(p, wp, f"{what}: param")
+    O.assert_bits(v, wv, f"{what}: exp_avg_sq")
+    O.assert_bits(p, wp, f"{what}: param")
 
 
 @pytest.mark.parametrize("wd", [0.0, 0.05])

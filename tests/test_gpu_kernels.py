@@ -39,22 +39,45 @@ def rand_coo(n_rows, n_cols, nnz, seed, dup_frac=0.1):
 
 
 # ------------------------------------------------------------------------------------------------ K1c
-@pytest.mark.parametrize("n_rows,n_cols,nnz", [(1, 1, 1), (7, 5, 0), (300, 200, 5000), (2000, 3000, 40000), (5, 100000, 3000)])
+@pytest.mark.parametrize("n_rows,n_cols,nnz", [(1, 1, 1), (7, 5, 0), (300, 200, 5000), (2000, 3000, 40000), (5, 100000, 3000),
+                                                (40, 1, 500), (65537, 65537, 4000), (1048573, 1048583, 3000)])
 def test_csr_from_coo_coalesce_semantics(dev, n_rows, n_cols, nnz):
+    """Bit for bit against `oracle.csr_coalesce_f32`: the documented stable sort, then a sequential fp32 sum of each run
+    in input order.  Every non-empty case also repeats one key 3 000 times with values of mixed sign and magnitude (so
+    the order shows in the bits); rows 0 and n_rows - 1 stay empty from 1 000 rows up; the last two cases span just
+    above 2^32 and about 2^40 keys (the radix sort's end bit); n_cols = 1 is all duplicates."""
     from mmrec_b200.ops import CSR
     r, c, v = rand_coo(n_rows, n_cols, nnz, seed=nnz + n_rows)
+    if n_rows >= 1000:
+        r = 1 + r % (n_rows - 2)
+    if nnz:
+        g = torch.Generator().manual_seed(n_rows)
+        rep = (torch.randn(3000, generator=g) * torch.exp2(torch.randint(-10, 10, (3000,), generator=g).float())).float()
+        at = torch.randint(0, r.numel() + 1, (3000,), generator=g).sort().values       # spread through the input
+        keep = torch.ones(r.numel() + 3000, dtype=torch.bool)
+        keep[at + torch.arange(3000)] = False
+        r2, c2, v2 = torch.empty(keep.numel(), dtype=r.dtype), torch.empty(keep.numel(), dtype=c.dtype), torch.empty(keep.numel())
+        r2[keep], c2[keep], v2[keep] = r, c, v
+        r2[~keep], c2[~keep], v2[~keep] = r[0], c[0], rep
+        r, c, v = r2, c2, v2
     A = CSR.from_coo(r.to(dev), c.to(dev), v.to(dev), n_rows, n_cols)
     ref = torch.sparse_coo_tensor(torch.stack([r, c]), v, (n_rows, n_cols)).coalesce()
     assert A.nnz == ref._nnz()
-    rp = A.rowptr.cpu().numpy()
-    assert rp[0] == 0 and rp[-1] == A.nnz and np.all(np.diff(rp) >= 0)
-    if A.nnz:
-        rows, cols, vals = [t.cpu() for t in A.coo()]
-        assert np.array_equal(torch.stack([rows, cols]).numpy(), ref.indices().numpy())       # row-major, sorted cols
-        np.testing.assert_allclose(vals.numpy(), ref.values().numpy(), rtol=1e-6, atol=1e-7)
-    # duplicates kept when asked
-    B = CSR.from_coo(r.to(dev), c.to(dev), None, n_rows, n_cols, sum_duplicates=False)
-    assert B.nnz == r.numel()
+    rowptr, colidx, vals = O.csr_coalesce_f32(r.numpy(), c.numpy(), v.numpy(), n_rows, n_cols)
+    assert np.array_equal(A.rowptr.cpu().numpy(), rowptr)
+    assert np.array_equal(A.colidx[:A.nnz].cpu().numpy(), colidx) and np.array_equal(colidx, ref.indices()[1].numpy())
+    O.assert_bits(A.vals[:A.nnz], vals, f"coalesced values {n_rows}x{n_cols}")
+    if n_rows >= 1000:
+        assert rowptr[1] == 0 and rowptr[-2] == rowptr[-1]
+    # val=None: every entry counts 1.0
+    B = CSR.from_coo(r.to(dev), c.to(dev), None, n_rows, n_cols)
+    O.assert_bits(B.vals[:B.nnz], O.csr_coalesce_f32(r.numpy(), c.numpy(), None, n_rows, n_cols)[2], "counts")
+    # duplicates kept when asked: equal keys in input order, values unchanged
+    D = CSR.from_coo(r.to(dev), c.to(dev), v.to(dev), n_rows, n_cols, sum_duplicates=False)
+    rowptr, colidx, vals = O.csr_coalesce_f32(r.numpy(), c.numpy(), v.numpy(), n_rows, n_cols, sum_duplicates=False)
+    assert D.nnz == r.numel() and np.array_equal(D.rowptr.cpu().numpy(), rowptr)
+    assert np.array_equal(D.colidx[:D.nnz].cpu().numpy(), colidx)
+    O.assert_bits(D.vals[:D.nnz], vals, "sum_duplicates=False")
 
 
 def test_csr_transpose_and_plan(dev):
@@ -530,49 +553,121 @@ def test_peer_gather_and_row_range_merge(dev):
     assert torch.equal(fv, v2) and torch.equal(fi, i2)
 
 
-def test_device_evaluator_matches_host_metrics(dev):
+class _EvalLoader:
+    def __init__(self, pos):
+        self.pos = pos
+
+    def get_eval_items(self):
+        return self.pos
+
+    def get_eval_len_list(self):
+        return np.array([len(p) for p in self.pos], dtype=np.int64)
+
+
+def _eval_case(K, profile, n, seed):
+    """Positive lists of the profile and top-K lists: users u % 3 == 0 hold every positive they can (all K positions when
+    pos_len >= K), u % 3 == 1 hold none, the others a random mix.  Item ids start at 2^33."""
+    rng = np.random.default_rng(seed)
+    I = 12000
+    lens = {"ones": np.ones(n, np.int64), "around_k": np.maximum(1, K - 1 + np.arange(n) % 3),
+            "triple_k": np.full(n, 3 * K), "mixed": rng.integers(1, 2 * K + 6, n)}.get(profile)
+    if profile == "long":
+        lens = rng.integers(1, 2 * K + 6, n)
+        lens[n // 2] = 5000
+    pos = [rng.choice(I, size=int(m), replace=False).astype(np.int64) for m in lens]
+    topk = np.empty((n, K), np.int64)
+    for u in range(n):
+        if u % 3 == 1:
+            topk[u] = rng.choice(np.setdiff1d(np.arange(I), pos[u]), K, replace=False)
+        else:
+            topk[u] = rng.choice(I, K, replace=False)
+            if u % 3 == 0:
+                h = min(len(pos[u]), K)
+                topk[u] = rng.permutation(np.concatenate([pos[u][:h], np.setdiff1d(topk[u], pos[u][:h])])[:K])
+    off = np.int64(1) << 33
+    return [p + off for p in pos], topk + off
+
+
+EVAL_KS = [1, 5, 31, 32, 33, 50, 64, 65, 100, 128]
+EVAL_PROFILES = [("ones", 9), ("around_k", 4099), ("triple_k", 7), ("long", 8), ("mixed", 1)]
+
+
+def test_device_evaluator_matches_host_metrics(dev, monkeypatch):
     """f2: mmrec_topk_metrics_f64 (hit matrix + Recall / NDCG / Precision / MAP sums on the device) against the numpy
     implementation of the reference's metric definitions (mmrec_b200/utils/topk_evaluator.py, pinned to the reference's
-    numbers by tests/test_oracle_golden.py)."""
-    from mmrec_b200.utils import topk_evaluator as TE
-
-    class Loader:
-        def __init__(self, pos):
-            self.pos = pos
-
-        def get_eval_items(self):
-            return self.pos
-
-        def get_eval_len_list(self):
-            return np.array([len(p) for p in self.pos], dtype=np.int64)
-
-    rng = np.random.default_rng(0)
-    n, I, K = 3001, 900, 50
-    pos = [rng.choice(I, size=rng.integers(1, 70), replace=False).astype(np.int64) for _ in range(n)]
-    topk = np.stack([rng.permutation(I)[:K] for _ in range(n)]).astype(np.int64)
-    for u in range(0, n, 7):                                # some users with many hits, some with a full list of hits
-        h = min(len(pos[u]), K)
-        topk[u, :h] = pos[u][:h]
-    cfg = {"metrics": ["Recall", "NDCG", "Precision", "MAP"], "topk": [5, 10, 20, 50], "device_evaluator": None}
-    ev = TE.TopKEvaluator(cfg)
-    batches = [torch.from_numpy(topk[lo:lo + 1024]).to(dev) for lo in range(0, n, 1024)]
-    got = ev.evaluate(batches, Loader(pos))
-    want = ev.evaluate([b.cpu() for b in batches], Loader(pos))
-    assert got.keys() == want.keys()
-    for key in want:
-        assert abs(got[key] - want[key]) <= 1.0001e-4, (key, got[key], want[key])      # both rounded to 4 decimals
-    # un-rounded: float64 sums in a different order
+    numbers by tests/test_oracle_golden.py), for every K of EVAL_KS and every (pos_len profile, n_users) of
+    EVAL_PROFILES.  K covers one to four 32-position rounds; pos_len sits at, below and above K (the `cap` of NDCG's
+    ideal DCG and of MAP's denominator) and far above it (the binary search); n covers partial and full 8-user CTAs;
+    batches of unequal size make every `ptr` slice start mid-array."""
     from mmrec_b200 import ops
+    calls = []
+    real = ops.topk_metric_sums
+    monkeypatch.setattr(ops, "topk_metric_sums", lambda *a: calls.append(1) or real(*a))
+    for K in EVAL_KS:
+        for profile, n in EVAL_PROFILES:
+            calls.clear()
+            _check_evaluator_case(dev, real, calls, K, profile, n)
+
+
+def _check_evaluator_case(dev, real, calls, K, profile, n):
+    """One case of test_device_evaluator_matches_host_metrics; `real` is the unpatched `ops.topk_metric_sums`, `calls`
+    counts the patched one's calls."""
+    from mmrec_b200.utils import topk_evaluator as TE
+    case = f"K={K} profile={profile} n={n}"
+    pos, topk = _eval_case(K, profile, n, seed=K * 31 + n)
+    cuts = sorted({0, n, *np.random.default_rng(K).integers(1, n, 2).tolist()} if n > 1 else {0, n})
+    batches = [torch.from_numpy(topk[lo:hi]).to(dev) for lo, hi in zip(cuts[:-1], cuts[1:])]
+    cfg = {"metrics": ["Recall", "NDCG", "Precision", "MAP"], "topk": sorted({1, (K + 1) // 2, K}), "device_evaluator": None}
+    ev = TE.TopKEvaluator(cfg)
+    got = ev.evaluate(batches, _EvalLoader(pos))
+    assert len(calls) == len(batches), case                 # the device route served every batch
+    want = ev.evaluate([b.cpu() for b in batches], _EvalLoader(pos))
+    assert len(calls) == len(batches) and got.keys() == want.keys(), case
+    # un-rounded: float64 sums in a different order
     hit = TE.hit_matrix(topk, pos)
     pos_len = np.array([len(p) for p in pos])
     disc = 1.0 / np.log2(np.arange(1, K + 1) + 1.0)
     ptr = torch.from_numpy(np.concatenate([[0], np.cumsum(pos_len)])).to(dev)
     items = torch.from_numpy(np.concatenate([np.sort(p) for p in pos])).to(dev)
     sums = torch.zeros(4, K, dtype=torch.float64, device=dev)
-    ops.topk_metric_sums(torch.from_numpy(topk).to(dev), ptr, items, torch.from_numpy(disc).to(dev), torch.from_numpy(np.cumsum(disc)).to(dev), sums)
+    real(torch.from_numpy(topk).to(dev), ptr, items, torch.from_numpy(disc).to(dev), torch.from_numpy(np.cumsum(disc)).to(dev), sums)
     mean = (sums / n).cpu().numpy()
-    for row, fn in enumerate((TE.recall_, TE.ndcg_, TE.precision_, TE.map_)):
-        np.testing.assert_allclose(mean[row], fn(hit, pos_len), rtol=1e-12, atol=1e-14)
+    host = {}
+    for row, (name, fn) in enumerate((("recall", TE.recall_), ("ndcg", TE.ndcg_), ("precision", TE.precision_), ("map", TE.map_))):
+        host[name] = fn(hit, pos_len)
+        np.testing.assert_allclose(mean[row], host[name], rtol=1e-12, atol=1e-14, err_msg=f"{case} {name}")
+    # rounded to 4 decimals: equal, except where the host's value lies within 1e-12 of a rounding midpoint (the device's
+    # atomic sums have no fixed order)
+    for key in want:
+        if got[key] != want[key]:
+            m, k = key.split("@")
+            v = float(host[m][int(k) - 1])
+            assert abs(v * 1e4 - np.floor(v * 1e4) - 0.5) * 1e-4 <= 1e-12, (case, key, got[key], want[key], v)
+
+
+@pytest.mark.parametrize("route", ["K=129", "recall2", "device_evaluator=False"])
+def test_evaluator_routes_to_the_host(dev, monkeypatch, route):
+    """K > 128, `recall2` and `device_evaluator: False` take the host route and give the host's numbers; the device entry
+    rejects K = 129."""
+    from mmrec_b200 import ops
+    from mmrec_b200._lib import MMRecError
+    from mmrec_b200.utils import topk_evaluator as TE
+    K = 129 if route == "K=129" else 20
+    pos, topk = _eval_case(K, "mixed", 50, seed=3)
+    calls = []
+    real = ops.topk_metric_sums
+    monkeypatch.setattr(ops, "topk_metric_sums", lambda *a: calls.append(1) or real(*a))
+    metrics = ["Recall", "NDCG", "Precision", "MAP"] + (["Recall2"] if route == "recall2" else [])
+    cfg = {"metrics": metrics, "topk": [1, K], "device_evaluator": False if route == "device_evaluator=False" else None}
+    ev = TE.TopKEvaluator(cfg)
+    got = ev.evaluate([torch.from_numpy(topk[:20]).to(dev), torch.from_numpy(topk[20:]).to(dev)], _EvalLoader(pos))
+    assert calls == []
+    assert got == ev.evaluate([torch.from_numpy(topk)], _EvalLoader(pos))
+    if route == "K=129":
+        disc = torch.ones(K, dtype=torch.float64, device=dev)
+        with pytest.raises(MMRecError):
+            real(torch.from_numpy(topk).to(dev), torch.zeros(51, dtype=torch.int64, device=dev), torch.zeros(1, dtype=torch.int64, device=dev),
+                 disc, disc, torch.zeros(4, K, dtype=torch.float64, device=dev))
 
 
 @pytest.mark.parametrize("d,L,mm_layers", [(64, 3, 1), (64, 1, 1), (128, 2, 2), (32, 4, 0), (64, 2, 0)])
