@@ -141,6 +141,21 @@ typedef struct {
 } mmrec_spmm_step;
 int mmrec_spmm_chain_f32(int d, int n_steps, const mmrec_spmm_step* steps, void* stream);
 
+/* The general form: mmrec_spmm_chain_f32 is this call with cooperative = 1 and no second blocks.
+ *   Second row blocks of the dense operands (nullable): X row c is X_hi[c - x_split, :] for c >= x_split, acc_in row r is
+ *   acc_in_hi[r - acc_in_split, :] for r >= acc_in_split (acc_in and acc_out must be set) -- layer 1 of a propagation reads
+ *   [users; items] straight from the two embedding tables, with the same bits as from their concatenation.
+ *   cooperative != 0: one cooperative launch, a grid barrier before every `sync_before` step.  cooperative == 0: the steps up
+ *   to the next `sync_before` step share one ordinary launch (steps that do not read each other's output, such as FREEDOM's
+ *   item-item product and layer 1 on A_hat); each `sync_before` step starts a new launch on the stream.  Steps of one launch
+ *   must not share a work plan's counters / partial buffer. */
+typedef struct {
+    mmrec_spmm_step step;
+    const float* X_hi; int64_t ldx_hi; int64_t x_split;                   /* nullable */
+    const float* acc_in_hi; int64_t ldacc_in_hi; int64_t acc_in_split;    /* nullable */
+} mmrec_spmm_step2;
+int mmrec_spmm_steps_f32(int d, int n_steps, const mmrec_spmm_step2* steps, int cooperative, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * K2  fused gather -> linear(+bias) -> optional row L2-normalise.   Replaces
  * `self.image_trs(self.image_embedding.weight)[items]` (src/models/freedom.py:205-209,

@@ -31,6 +31,7 @@ PROTOTYPES = {
     "mmrec_spmm_acc_f32": (_i32, [_i64, _i64, _i32, _p, _p, _p, _p, _i64, _i64, _p, _p, _p, _p, _i64, _p, _i64, _p, _p, _i64,
                                   _f32, _i32, _p]),
     "mmrec_spmm_chain_f32": (_i32, [_i32, _i32, _p, _p]),
+    "mmrec_spmm_steps_f32": (_i32, [_i32, _i32, _p, _i32, _p]),
     "mmrec_project_set_path": (_i32, [_i32]),
     "mmrec_project_workspace_bytes": (_sz, [_i64, _i64, _i32]),
     "mmrec_project_f32": (_i32, [_i64, _p, _p, _i64, _i64, _p, _p, _i32, _i32, _p, _i64, _p, _sz, _p]),
@@ -81,6 +82,12 @@ class SpmmStep(C.Structure):
                 ("X", _p), ("ldx", _i64), ("Y", _p), ("ldy", _i64),
                 ("acc_in", _p), ("acc_out", _p), ("ldacc", _i64), ("acc_div", _f32),
                 ("post", _p), ("ldpost", _i64), ("post_row0", _i64), ("sync_before", _i32)]
+
+
+class SpmmStep2(C.Structure):
+    """`mmrec_spmm_step2` of include/mmrec_b200.h: a step plus the second row blocks of X and acc_in."""
+    _fields_ = [("step", SpmmStep), ("X_hi", _p), ("ldx_hi", _i64), ("x_split", _i64),
+                ("acc_in_hi", _p), ("ldacc_in_hi", _i64), ("acc_in_split", _i64)]
 
 
 class AdamTensor(C.Structure):

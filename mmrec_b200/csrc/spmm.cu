@@ -35,6 +35,12 @@ struct SpmmParams {
     const float* post; int64_t post_row0; uint32_t spost;   // acc_out[r,:] += post[r - post_row0, :] for r >= post_row0 (after the division)
     int d;
     uint32_t sx, sy, sacc, sgate;      // the leading dimensions as byte strides (vector kernel: one IMAD.WIDE per row address)
+    // Two-block operands (chained kernel only, mmrec_spmm_steps_f32): row c of X is X_hi[c - x_split] for c >= x_split, row r of
+    // acc_in is acc_in_hi[r - acc_split] for r >= acc_split -- [users; items] straight from the two embedding tables, no copy.
+    // One block: X_hi = X, x_split = n_cols, acc_in_hi = acc_in, acc_split = n_rows.
+    const float* X_hi; const float* acc_in_hi;
+    int x_split, acc_split;
+    uint32_t sx_hi, sacc_hi;
 };
 
 // T lanes cooperate on one task (row or row segment); a warp runs 32/T tasks at once.  Fewer lanes per row
@@ -47,6 +53,13 @@ __device__ __forceinline__ const float4* row_f4(const float* base, uint32_t stri
 }
 __device__ __forceinline__ float4* row_f4(float* base, uint32_t stride, int r, int f4) {
     return reinterpret_cast<float4*>(reinterpret_cast<char*>(base) + (uint64_t)(uint32_t)r * stride) + f4;
+}
+
+// Row `r` of acc_in; TWO: from the block the row falls in (a select, not a branch: the lane groups of a warp may straddle the split).
+template <bool TWO>
+__device__ __forceinline__ float4 acc_in_f4(const SpmmParams& p, int r, int f4) {
+    const bool hi = TWO && r >= p.acc_split;
+    return *row_f4(hi ? p.acc_in_hi : p.acc_in, hi ? p.sacc_hi : p.sacc, hi ? r - p.acc_split : r, f4);
 }
 
 template <int D, int T>
@@ -117,13 +130,16 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmParams& p, bool on, int 
 
 // Gather of one task range [b, b + len) by one lane group: UNR rows of X in flight, the next batch's indices
 // travel while they are.  `maxlen` is the trip bound shared by every group that runs in lock step with this one.
-template <int D, int T>
+// TWO: each gathered row is read from the block of X it falls in; the products and their order are the same as from the
+// concatenation, so the result is bit-identical.
+template <int D, int T, bool TWO>
 __device__ __forceinline__ void spmm_gather(const SpmmParams& p, int b, int len, int maxlen, int l, float4 (&acc)[VecCfg<D, T>::V]) {
     using C = VecCfg<D, T>;
     int cj[C::UNR]; float wj[C::UNR];
     const int32_t* cp = p.colidx + b;                                // walked with immediate offsets: no per-load address math
     const float* vp = p.vals + b;
     const float* xl = p.X + l * 4;
+    const float* xh = TWO ? p.X_hi + l * 4 : xl;
 #pragma unroll
     for (int u = 0; u < C::UNR; ++u) {
         const bool ok = u < len;
@@ -135,9 +151,13 @@ __device__ __forceinline__ void spmm_gather(const SpmmParams& p, int b, int len,
 #pragma unroll
         for (int u = 0; u < C::UNR; ++u) {
             const bool ok = j0 + u < len;
+            const bool hi = TWO && cj[u] >= p.x_split;
+            const float* xb = hi ? xh : xl;
+            const uint32_t sb = hi ? p.sx_hi : p.sx;
+            const int rb = hi ? cj[u] - p.x_split : cj[u];
 #pragma unroll
             for (int v = 0; v < C::V; ++v)
-                x[u][v] = ok ? __ldg(row_f4(xl, p.sx, cj[u], v * T)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                x[u][v] = ok ? __ldg(row_f4(xb, sb, rb, v * T)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
         float wc[C::UNR];
 #pragma unroll
@@ -164,7 +184,7 @@ __device__ __forceinline__ void spmm_gather(const SpmmParams& p, int b, int len,
 // A finished task of a split row: publish the partial, and if this is the last segment of the row to arrive, add
 // the partials in segment order and return true (the caller then runs the epilogue).  Warp-collective (full mask);
 // `split` marks the lane groups that hold such a task.
-template <int D, int T>
+template <int D, int T, bool TWO>
 __device__ __forceinline__ bool spmm_split_finish(const SpmmParams& p, bool split, int row, int b, int sid, int l,
                                                   float4 (&acc)[VecCfg<D, T>::V], float4 (&accin)[VecCfg<D, T>::V]) {
     using C = VecCfg<D, T>;
@@ -208,7 +228,7 @@ __device__ __forceinline__ bool spmm_split_finish(const SpmmParams& p, bool spli
         if (p.acc_in) {
 #pragma unroll
             for (int v = 0; v < C::V; ++v)
-                accin[v] = *row_f4(p.acc_in, p.sacc, row, v * T + l);
+                accin[v] = acc_in_f4<TWO>(p, row, v * T + l);
         }
         if (l == 0) p.counters[sid] = 0;                    // self-cleaning for the next launch
         last = true;
@@ -225,7 +245,7 @@ __device__ __forceinline__ bool spmm_split_finish(const SpmmParams& p, bool spli
 // predicated, no shuffles in the gather loop (the T lanes of a group read the same (col, val) address = one
 // broadcast transaction).  Warps walk the sorted list boustrophedon, so whoever got the longest tasks in one sweep
 // gets the shortest in the next.
-template <int D, int T>
+template <int D, int T, bool TWO>
 __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __restrict__ red) {
     using C = VecCfg<D, T>;
     constexpr int G = 256 / T;                              // lane groups per CTA
@@ -250,12 +270,12 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
         if (warp == 0 && g == 0 && p.acc_in && sid < 0) {
 #pragma unroll
             for (int v = 0; v < C::V; ++v)
-                accin[v] = *row_f4(p.acc_in, p.sacc, row, v * T + l);
+                accin[v] = acc_in_f4<TWO>(p, row, v * T + l);
         }
         float4 acc[C::V];
 #pragma unroll
         for (int v = 0; v < C::V; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-        spmm_gather<D, T>(p, mb, mylen, chunk, l, acc);
+        spmm_gather<D, T, TWO>(p, mb, mylen, chunk, l, acc);
 #pragma unroll
         for (int v = 0; v < C::V; ++v) *reinterpret_cast<float4*>(red + gi * D + (v * T + l) * 4) = acc[v];
         __syncthreads();
@@ -272,7 +292,7 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
                 }
             }
             bool do_epi = g == 0 && sid < 0;
-            if (sid >= 0) do_epi = spmm_split_finish<D, T>(p, g == 0, row, tk.y, sid, l, acc, accin);
+            if (sid >= 0) do_epi = spmm_split_finish<D, T, TWO>(p, g == 0, row, tk.y, sid, l, acc, accin);
             spmm_epilogue<D, T>(p, do_epi, row, l, acc, accin);
         }
         __syncthreads();
@@ -304,16 +324,16 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
         if (valid && p.acc_in && sid < 0) {                         // epilogue operand does not depend on the gather
 #pragma unroll
             for (int v = 0; v < C::V; ++v)
-                accin[v] = *row_f4(p.acc_in, p.sacc, row, v * T + l);
+                accin[v] = acc_in_f4<TWO>(p, row, v * T + l);
         }
         float4 acc[C::V];
 #pragma unroll
         for (int v = 0; v < C::V; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-        spmm_gather<D, T>(p, b, valid ? len : 0, maxlen, l, acc);
+        spmm_gather<D, T, TWO>(p, b, valid ? len : 0, maxlen, l, acc);
         bool do_epi = valid && sid < 0;
         const bool split = valid && sid >= 0;
         if (__any_sync(0xffffffffu, split)) {
-            if (spmm_split_finish<D, T>(p, split, row, b, sid, l, acc, accin)) do_epi = true;
+            if (spmm_split_finish<D, T, TWO>(p, split, row, b, sid, l, acc, accin)) do_epi = true;
         }
         spmm_epilogue<D, T>(p, do_epi, row, l, acc, accin);
     }
@@ -322,23 +342,22 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
 template <int D, int T>
 __global__ void __launch_bounds__(256) spmm_vec_kernel(const SpmmParams p) {
     __shared__ __align__(16) float red[(256 / T) * D];
-    spmm_vec_body<D, T>(p, red);
+    spmm_vec_body<D, T, false>(p, red);
 }
 
-// A chain of SpMMs in ONE persistent cooperative launch: the steps run in order on the same resident grid, a grid-wide
-// barrier wherever a step reads what an earlier one wrote (`sync_mask`).  The propagation of one `forward` -- L layers
-// on A_hat plus the item-item layer -- is one launch instead of L + 1: at Amazon-scale graphs a layer is a handful of
-// dependent L2 round trips, and launch ramp + tail of every layer were a third of its time.
+// Several SpMMs in one persistent launch: the steps run in order on the same grid, a CTA that is done with one step starts
+// the next, so the tail of one step overlaps the work of the next.  COOP (a cooperative launch, every CTA resident): a
+// grid-wide barrier before every step of `sync_mask` (it reads what an earlier step wrote), so a whole propagation is one
+// launch.  Without COOP the steps of one launch must be independent -- FREEDOM's item-item product beside layer 1 on A_hat.
 constexpr int SPMM_CHAIN_MAX = 8;
 struct SpmmChain { SpmmParams step[SPMM_CHAIN_MAX]; int n; unsigned sync_mask; };
 
-template <int D, int T>
-__global__ void __launch_bounds__(256) spmm_chain_kernel(const SpmmChain c) {
+template <int D, int T, bool COOP>
+__global__ void __launch_bounds__(256, 3) spmm_chain_kernel(const SpmmChain c) {
     __shared__ __align__(16) float red[(256 / T) * D];
-    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
     for (int i = 0; i < c.n; ++i) {
-        if ((c.sync_mask >> i) & 1u) { __threadfence(); grid.sync(); }
-        spmm_vec_body<D, T>(c.step[i], red);
+        if (COOP && ((c.sync_mask >> i) & 1u)) { __threadfence(); cooperative_groups::this_grid().sync(); }
+        spmm_vec_body<D, T, true>(c.step[i], red);
     }
 }
 
@@ -448,6 +467,7 @@ extern "C" int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d, const int32
     MMREC_CHECK_ARG(ldx < (1ll << 30) && ldy < (1ll << 30) && ldacc < (1ll << 30) && ldgate < (1ll << 30) && n_cols < (1ll << 31) &&
                     n_rows < (1ll << 31), "spmm: leading dimension / size out of range");
     p.sx = (uint32_t)(ldx * 4); p.sy = (uint32_t)(ldy * 4); p.sacc = (uint32_t)(ldacc * 4); p.sgate = (uint32_t)(ldgate * 4);
+    p.X_hi = X; p.x_split = (int)n_cols; p.sx_hi = p.sx; p.acc_in_hi = acc_in; p.acc_split = (int)n_rows; p.sacc_hi = p.sacc;
     auto al16 = [](const void* q, int64_t ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld & 3) == 0); };
     const bool vec_ok = al16(X, ldx) && al16(Y, ldy) && al16(acc_in, ldacc) && al16(acc_out, ldacc) &&
                         al16(gate_ref, ldgate) && al16(partial, 4);
@@ -484,48 +504,90 @@ extern "C" int mmrec_spmm_acc_f32(int64_t n_rows, int64_t n_cols, int d, const i
 }
 
 namespace mmrec {
-template <int D>
-static int launch_chain(const SpmmChain& c, int64_t max_work, cudaStream_t stream) {
+// One launch of the chained kernel; COOP: cooperative, so that every CTA is resident for the grid barriers.
+template <int D, bool COOP>
+static int launch_chain(const SpmmChain& c, cudaStream_t stream) {
     constexpr int T = D / 4 > 32 ? 32 : D / 4;                       // one float4 per lane, as the single-step default
     static int blocks_per_sm = 0;
     if (!blocks_per_sm) {
-        MMREC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, spmm_chain_kernel<D, T>, 256, 0));
+        MMREC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, spmm_chain_kernel<D, T, COOP>, 256, 0));
         if (blocks_per_sm < 1) blocks_per_sm = 1;
+    }
+    int64_t max_work = 1;
+    for (int i = 0; i < c.n; ++i) {
+        const int64_t work = c.step[i].n_tasks > c.step[i].n_heavy ? c.step[i].n_tasks : c.step[i].n_heavy * 8;
+        if (work > max_work) max_work = work;
     }
     const int per_block = 8 * (32 / T);
     int64_t grid = (max_work + per_block - 1) / per_block;
-    const int64_t cap = (int64_t)sm_count() * blocks_per_sm;         // every block resident: the grid barrier needs it
+    const int64_t cap = (int64_t)sm_count() * blocks_per_sm;         // every block resident (the grid barrier needs it)
     if (grid > cap) grid = cap;
     if (grid < 1) grid = 1;
-    void* args[] = {(void*)&c};
-    MMREC_CUDA(cudaLaunchCooperativeKernel((const void*)spmm_chain_kernel<D, T>, dim3((unsigned)grid), dim3(256), args, 0, stream));
-    ++g_launches;
+    if (COOP) {
+        void* args[] = {(void*)&c};
+        MMREC_CUDA(cudaLaunchCooperativeKernel((const void*)spmm_chain_kernel<D, T, true>, dim3((unsigned)grid), dim3(256), args, 0, stream));
+        ++g_launches;
+    } else {
+        spmm_chain_kernel<D, T, false><<<(unsigned)grid, 256, 0, stream>>>(c);
+        MMREC_LAUNCH_CHECK();
+    }
+    return MMREC_OK;
+}
+
+// Without the cooperative launch, each run of steps up to the next `sync_before` is one ordinary launch; a run of one step
+// with one-block operands is the single-SpMM kernel (the chained kernel reads its parameters by a run-time step index).
+template <int D>
+static int launch_steps(const SpmmChain& c, int cooperative, cudaStream_t stream) {
+    if (cooperative) return launch_chain<D, true>(c, stream);
+    constexpr int T = D / 4 > 32 ? 32 : D / 4;
+    for (int i = 0; i < c.n;) {
+        int j = i + 1;
+        while (j < c.n && !((c.sync_mask >> j) & 1u)) ++j;
+        const SpmmParams& p = c.step[i];
+        int rc;
+        if (j == i + 1 && p.x_split == p.n_cols && p.acc_split == p.n_rows) {
+            rc = launch_vec<D, T>(p, stream);
+        } else {
+            SpmmChain run;
+            run.n = j - i; run.sync_mask = 0;
+            for (int k = 0; k < run.n; ++k) run.step[k] = c.step[i + k];
+            rc = launch_chain<D, false>(run, stream);
+        }
+        if (rc != MMREC_OK) return rc;
+        i = j;
+    }
     return MMREC_OK;
 }
 }  // namespace mmrec
 
-extern "C" int mmrec_spmm_chain_f32(int d, int n_steps, const mmrec_spmm_step* steps, void* stream_) {
+extern "C" int mmrec_spmm_steps_f32(int d, int n_steps, const mmrec_spmm_step2* steps, int cooperative, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
-    MMREC_CHECK_ARG(n_steps >= 1 && n_steps <= SPMM_CHAIN_MAX && steps, "spmm_chain: 1 <= n_steps <= %d", SPMM_CHAIN_MAX);
+    MMREC_CHECK_ARG(n_steps >= 1 && n_steps <= SPMM_CHAIN_MAX && steps, "spmm_steps: 1 <= n_steps <= %d", SPMM_CHAIN_MAX);
     if (!(d == 32 || d == 64 || d == 128 || d == 256) || g_spmm_lanes) {
-        set_error("spmm_chain: d = %d (or a lane override) has no chained kernel; launch the steps one by one", d);
+        set_error("spmm_steps: d = %d (or a lane override) has no chained kernel; launch the steps one by one", d);
         return MMREC_EUNSUPPORTED;
     }
     SpmmChain c;
     c.n = n_steps; c.sync_mask = 0;
-    int64_t max_work = 1;
     auto al16 = [](const void* q, int64_t ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld & 3) == 0); };
     for (int i = 0; i < n_steps; ++i) {
-        const mmrec_spmm_step& t = steps[i];
-        MMREC_CHECK_ARG(t.n_rows >= 0 && t.n_cols >= 0 && t.rowptr && t.X && (t.Y || t.acc_out), "spmm_chain: step %d: null pointer / bad sizes", i);
+        const mmrec_spmm_step& t = steps[i].step;
+        const mmrec_spmm_step2& t2 = steps[i];
+        MMREC_CHECK_ARG(t.n_rows >= 0 && t.n_cols >= 0 && t.rowptr && t.X && (t.Y || t.acc_out), "spmm_steps: step %d: null pointer / bad sizes", i);
         MMREC_CHECK_ARG(t.tasks && t.n_tasks >= 0 && t.n_cta_tasks >= 0 && t.n_cta_tasks <= t.n_tasks && t.split_rows && t.counters && t.partial,
-                        "spmm_chain: step %d: the chained kernel needs the work plan (mmrec_spmm_plan)", i);
+                        "spmm_steps: step %d: the chained kernel needs the work plan (mmrec_spmm_plan)", i);
         MMREC_CHECK_ARG(t.ldx >= d && (!t.Y || t.ldy >= d) && (!t.acc_out || t.ldacc >= d) && (!t.post || t.ldpost >= d) && t.acc_div != 0.0f,
-                        "spmm_chain: step %d: leading dimension < d or acc_div == 0", i);
+                        "spmm_steps: step %d: leading dimension < d or acc_div == 0", i);
         MMREC_CHECK_ARG(t.ldx < (1ll << 30) && t.ldy < (1ll << 30) && t.ldacc < (1ll << 30) && t.ldpost < (1ll << 30) && t.n_cols < (1ll << 31) &&
-                        t.n_rows < (1ll << 31), "spmm_chain: step %d: size out of range", i);
-        if (!(al16(t.X, t.ldx) && al16(t.Y, t.ldy) && al16(t.acc_in, t.ldacc) && al16(t.acc_out, t.ldacc) && al16(t.post, t.ldpost) && al16(t.partial, 4))) {
-            set_error("spmm_chain: step %d: operands not 16-byte aligned; launch the steps one by one", i);
+                        t.n_rows < (1ll << 31), "spmm_steps: step %d: size out of range", i);
+        MMREC_CHECK_ARG(!t2.X_hi || (t2.x_split >= 0 && t2.x_split <= t.n_cols && t2.ldx_hi >= d && t2.ldx_hi < (1ll << 30)),
+                        "spmm_steps: step %d: X_hi needs 0 <= x_split <= n_cols and d <= ldx_hi < 2^30", i);
+        MMREC_CHECK_ARG(!t2.acc_in_hi || (t.acc_in && t.acc_out && t2.acc_in_split >= 0 && t2.acc_in_split <= t.n_rows && t2.ldacc_in_hi >= d &&
+                                          t2.ldacc_in_hi < (1ll << 30)),
+                        "spmm_steps: step %d: acc_in_hi needs acc_in, acc_out, 0 <= acc_in_split <= n_rows and d <= ldacc_in_hi < 2^30", i);
+        if (!(al16(t.X, t.ldx) && al16(t.Y, t.ldy) && al16(t.acc_in, t.ldacc) && al16(t.acc_out, t.ldacc) && al16(t.post, t.ldpost) && al16(t.partial, 4) &&
+              al16(t2.X_hi, t2.ldx_hi) && al16(t2.acc_in_hi, t2.ldacc_in_hi))) {
+            set_error("spmm_steps: step %d: operands not 16-byte aligned; launch the steps one by one", i);
             return MMREC_EUNSUPPORTED;
         }
         SpmmParams& p = c.step[i];
@@ -535,14 +597,25 @@ extern "C" int mmrec_spmm_chain_f32(int d, int n_steps, const mmrec_spmm_step* s
         p.acc_in = t.acc_in; p.acc_out = t.acc_out; p.ldacc = t.ldacc; p.acc_div = t.acc_div; p.gate_ref = nullptr; p.ldgate = 0;
         p.post = t.post; p.post_row0 = t.post_row0; p.d = d; p.y_acc = 0;
         p.sx = (uint32_t)(t.ldx * 4); p.sy = (uint32_t)(t.ldy * 4); p.sacc = (uint32_t)(t.ldacc * 4); p.sgate = 0; p.spost = (uint32_t)(t.ldpost * 4);
+        p.X_hi = t2.X_hi ? t2.X_hi : t.X;
+        p.x_split = (int)(t2.X_hi ? t2.x_split : t.n_cols);
+        p.sx_hi = (uint32_t)((t2.X_hi ? t2.ldx_hi : t.ldx) * 4);
+        p.acc_in_hi = t2.acc_in_hi ? t2.acc_in_hi : t.acc_in;
+        p.acc_split = (int)(t2.acc_in_hi ? t2.acc_in_split : t.n_rows);
+        p.sacc_hi = (uint32_t)((t2.acc_in_hi ? t2.ldacc_in_hi : t.ldacc) * 4);
         if (t.sync_before && i > 0) c.sync_mask |= 1u << i;
-        const int64_t work = t.n_tasks > t.n_cta_tasks ? t.n_tasks : t.n_cta_tasks * 8;
-        if (work > max_work) max_work = work;
     }
     switch (d) {
-        case 32: return launch_chain<32>(c, max_work, stream);
-        case 64: return launch_chain<64>(c, max_work, stream);
-        case 128: return launch_chain<128>(c, max_work, stream);
-        default: return launch_chain<256>(c, max_work, stream);
+        case 32: return launch_steps<32>(c, cooperative, stream);
+        case 64: return launch_steps<64>(c, cooperative, stream);
+        case 128: return launch_steps<128>(c, cooperative, stream);
+        default: return launch_steps<256>(c, cooperative, stream);
     }
+}
+
+extern "C" int mmrec_spmm_chain_f32(int d, int n_steps, const mmrec_spmm_step* steps, void* stream_) {
+    MMREC_CHECK_ARG(n_steps >= 1 && n_steps <= SPMM_CHAIN_MAX && steps, "spmm_chain: 1 <= n_steps <= %d", SPMM_CHAIN_MAX);
+    mmrec_spmm_step2 s2[SPMM_CHAIN_MAX] = {};
+    for (int i = 0; i < n_steps; ++i) s2[i].step = steps[i];
+    return mmrec_spmm_steps_f32(d, n_steps, s2, 1, stream_);
 }

@@ -43,8 +43,10 @@ class BM3(GeneralRecommender):
 
     def forward(self):
         h = self.item_id_embedding.weight
-        ego = torch.cat((self.user_embedding.weight, h), dim=0)
-        all_emb = ops.propagate_mean(self.norm_adj, ego, self.n_layers)
+        if not torch.is_grad_enabled() and h.is_cuda:                # inference: the layers read the two tables in place
+            all_emb = ops.propagate_mean_fused(self.norm_adj, (self.user_embedding.weight, h), self.n_layers, cooperative=False)
+        else:
+            all_emb = ops.propagate_mean(self.norm_adj, torch.cat((self.user_embedding.weight, h), dim=0), self.n_layers)
         u_g, i_g = torch.split(all_emb, [self.n_users, self.n_items], dim=0)
         return u_g, i_g + h
 

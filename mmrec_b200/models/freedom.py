@@ -59,12 +59,15 @@ class FREEDOM(GeneralRecommender):
         self.masked_adj, _ = self.pruner.sample(self.dropout)
 
     def forward(self, adj):
-        ego = torch.cat((self.user_embedding.weight, self.item_id_embedding.weight), dim=0)
-        if ops.CHAIN and not torch.is_grad_enabled() and self.n_layers >= 1 and self.n_ui_layers >= 1:
-            # inference: the item-item product(s), the UI layers, the layer mean and `i_g + h` in one cooperative launch
-            all_emb = ops.propagate_mean_fused(adj, ego, self.n_ui_layers, post_csr=self.mm_adj, post_x=self.item_id_embedding.weight,
-                                               post_layers=self.n_layers, post_row0=self.n_users)
+        user_w, item_w = self.user_embedding.weight, self.item_id_embedding.weight
+        if not torch.is_grad_enabled() and user_w.is_cuda and self.n_layers >= 1 and self.n_ui_layers >= 1:
+            # inference: layer 1 reads the two tables in place (no concatenated copy), the item-item product shares its launch,
+            # `i_g + h` rides in the last layer's epilogue -- n_ui_layers ordinary launches.  (One cooperative launch with grid
+            # barriers instead measured slower on the H100.)
+            all_emb = ops.propagate_mean_fused(adj, (user_w, item_w), self.n_ui_layers, post_csr=self.mm_adj, post_x=item_w,
+                                               post_layers=self.n_layers, post_row0=self.n_users, cooperative=False)
             return torch.split(all_emb, [self.n_users, self.n_items], dim=0)
+        ego = torch.cat((user_w, item_w), dim=0)
         all_emb = ops.propagate_mean(adj, ego, self.n_ui_layers)
         u_g, i_g = torch.split(all_emb, [self.n_users, self.n_items], dim=0)
         if self.n_layers == 0:

@@ -57,7 +57,10 @@ class MGCN(GeneralRecommender):
         item_w = self.item_id_embedding.weight
         image_feats = ops.project(self.image_embedding.weight, self.image_trs.weight, self.image_trs.bias)
         text_feats = ops.project(self.text_embedding.weight, self.text_trs.weight, self.text_trs.bias)
-        content = ops.propagate_mean(adj, torch.cat([self.user_embedding.weight, item_w], dim=0), self.n_ui_layers)
+        if item_w.is_cuda:                                           # the layers read the two tables in place
+            content = ops.propagate_mean_fused(adj, (self.user_embedding.weight, item_w), self.n_ui_layers, cooperative=False)
+        else:
+            content = ops.propagate_mean(adj, torch.cat([self.user_embedding.weight, item_w], dim=0), self.n_ui_layers)
         views = []
         for feats, gate, knn in ((image_feats, self.gate_v, self.image_original_adj), (text_feats, self.gate_t, self.text_original_adj)):
             emb = torch.empty(U + self.n_items, d, dtype=torch.float32, device=item_w.device)

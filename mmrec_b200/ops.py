@@ -18,9 +18,6 @@ _ws_cache: dict = {}
 import os as _os
 SEG = int(_os.environ.get("MMREC_SPMM_SEG", "512"))        # non-zeros per SpMM task (rows longer than this are split)
 LIGHT_MAX = int(_os.environ.get("MMREC_SPMM_LIGHT", "32"))  # tasks longer than this are run by a whole CTA
-# All SpMMs of an inference-time propagation in one cooperative launch (mmrec_spmm_chain_f32).  Opt-in: a grid-wide barrier
-# per layer is not cheaper than the launch boundary it replaces when the launches are replayed from a CUDA graph.
-CHAIN = _os.environ.get("MMREC_SPMM_CHAIN", "0") == "1"
 
 
 def launch_count() -> int:
@@ -279,58 +276,86 @@ def spmm(A: CSR, X: torch.Tensor, base: Optional[torch.Tensor] = None) -> torch.
 
 
 def _chain_step(A: CSR, X, Y=None, acc_in=None, acc_out=None, acc_div=1.0, post=None, post_row0=0, sync_before=False):
-    d = X.shape[1]
-    st = _lib.SpmmStep()
+    """One `mmrec_spmm_step2`.  X and acc_in are a tensor or a (rows below the split, rows from the split on) pair."""
+    st2 = _lib.SpmmStep2()
+    st = st2.step
+    X_lo, X_hi = X if isinstance(X, tuple) else (X, None)
+    in_lo, in_hi = acc_in if isinstance(acc_in, tuple) else (acc_in, None)
+    d = X_lo.shape[1]
     st.n_rows, st.n_cols = A.n_rows, A.n_cols
     st.rowptr, st.colidx, st.vals = _ptr(A.rowptr), _ptr(A.colidx), _ptr(A.vals)
     st.tasks, st.n_tasks, st.n_cta_tasks = _ptr(A.tasks), A.n_tasks, A.n_cta_tasks
     st.split_rows, st.counters, st.partial = _ptr(A.split_rows), _ptr(A.counters), _ptr(A.partial(d))
-    st.X, st.ldx = _ptr(X), X.stride(0)
+    st.X, st.ldx = _ptr(X_lo), X_lo.stride(0)
     st.Y, st.ldy = _ptr(Y), d
-    st.acc_in, st.acc_out, st.ldacc, st.acc_div = _ptr(acc_in), _ptr(acc_out), d, float(acc_div)
+    st.acc_in, st.acc_out, st.ldacc, st.acc_div = _ptr(in_lo), _ptr(acc_out), d, float(acc_div)
     st.post, st.ldpost, st.post_row0 = _ptr(post), d, int(post_row0)
     st.sync_before = int(bool(sync_before))
-    return st
+    if X_hi is not None:
+        st2.X_hi, st2.ldx_hi, st2.x_split = _ptr(X_hi), X_hi.stride(0), X_lo.shape[0]
+    if in_hi is not None:
+        st2.acc_in_hi, st2.ldacc_in_hi, st2.acc_in_split = _ptr(in_hi), in_hi.stride(0), in_lo.shape[0]
+    return st2
 
 
-def propagate_mean_fused(A: CSR, ego: torch.Tensor, n_layers: int, post_csr: Optional[CSR] = None, post_x: Optional[torch.Tensor] = None,
-                         post_layers: int = 1, post_row0: int = 0) -> torch.Tensor:
-    """Inference form of `propagate_mean` (+ FREEDOM / BM3's item-item term) as ONE persistent cooperative launch
-    (`mmrec_spmm_chain_f32`): `mean(E_0 .. E_L)`, and if `post_csr` is given `out[post_row0:] += post_csr^post_layers @ post_x`
-    (`src/models/freedom.py:164-178`: `h = mm_adj @ ... @ item_emb`, `i_g + h`).  No autograd.  Falls back to one launch per
-    SpMM when the chained kernel does not take the shape."""
+def propagate_mean_fused(A: CSR, ego, n_layers: int, post_csr: Optional[CSR] = None, post_x: Optional[torch.Tensor] = None,
+                         post_layers: int = 1, post_row0: int = 0, cooperative: bool = True) -> torch.Tensor:
+    """Inference form of `propagate_mean` (+ FREEDOM / BM3's item-item term) through `mmrec_spmm_steps_f32`:
+    `mean(E_0 .. E_L)`, and if `post_csr` is given `out[post_row0:] += post_csr^post_layers @ post_x`
+    (`src/models/freedom.py:164-178`: `h = mm_adj @ ... @ item_emb`, `i_g + h`).  No autograd.
+
+    `ego` is E_0 as one tensor or as the pair (user table, item table): layer 1 then gathers from the two tables and adds
+    them to the running sum where they are, bit-identical to propagating their concatenation without making it.
+    `cooperative`: all steps in one cooperative launch with grid barriers; otherwise one ordinary launch per group of
+    independent steps (the item-item product shares layer 1's launch, each later layer is one launch).  Falls back to one
+    launch per SpMM when the chained kernel does not take the shape."""
     import ctypes
-    _need_cuda(ego, post_x)
-    ego = _f32c(ego)
-    d = ego.shape[1]
+    pair = isinstance(ego, (tuple, list))
+    parts = [_f32c(t) for t in ego] if pair else [_f32c(ego)]
+    _need_cuda(*parts, post_x)
+    d = parts[0].shape[1]
+    n = sum(t.shape[0] for t in parts)
+    if pair and any(t.shape[1] != d for t in parts):
+        raise MMRecError("propagate_mean_fused: the two tables differ in width")
+    if n != A.n_rows or n != A.n_cols:
+        raise MMRecError(f"propagate_mean_fused: E_0 has {n} rows, the matrix is {A.n_rows} x {A.n_cols}")
+    e0 = tuple(parts) if pair else parts[0]
+
+    def unfused():
+        return _propagate_mean_post_unfused(A, torch.cat(parts) if pair else parts[0], n_layers, post_csr, post_x, post_layers, post_row0)
+
     if n_layers < 1 or A.n_tasks == 0 or (post_csr is not None and post_csr.n_tasks == 0):
-        return _propagate_mean_post_unfused(A, ego, n_layers, post_csr, post_x, post_layers, post_row0)
-    steps, keep = [], []
+        return unfused()
+    # wave = how many launch boundaries (or grid barriers) must precede a step: h_i = post_csr @ h_{i-1} waits for h_{i-1},
+    # layer l for layer l - 1, and the last layer, whose epilogue adds h, also for the last item-item product
+    waves, keep = [], []
     h = None
     if post_csr is not None:
         h = _f32c(post_x)
         for i in range(post_layers):                                 # h = mm_adj @ h, the first one reads the parameters only
-            y = torch.empty(post_csr.n_rows, d, dtype=torch.float32, device=ego.device)
-            steps.append(_chain_step(post_csr, h, Y=y, sync_before=i > 0))
+            y = torch.empty(post_csr.n_rows, d, dtype=torch.float32, device=parts[0].device)
+            waves.append((i, 1, post_csr, dict(X=h, Y=y)))
             keep.append(y)
             h = y
-    acc = torch.empty_like(ego)
-    x = ego
+    acc = torch.empty(n, d, dtype=torch.float32, device=parts[0].device)
+    x = e0
     for l in range(1, n_layers + 1):
         last = l == n_layers
-        y = None if last else torch.empty_like(ego)
-        steps.append(_chain_step(A, x, Y=y, acc_in=ego if l == 1 else acc, acc_out=acc, acc_div=float(n_layers + 1) if last else 1.0,
-                                 post=h if last else None, post_row0=post_row0,
-                                 sync_before=(l > 1) or (last and h is not None)))
+        y = None if last else torch.empty_like(acc)
+        wave = max(l - 1, post_layers) if (last and h is not None) else l - 1
+        waves.append((wave, 0, A, dict(X=x, Y=y, acc_in=e0 if l == 1 else acc, acc_out=acc,
+                                       acc_div=float(n_layers + 1) if last else 1.0, post=h if last else None, post_row0=post_row0)))
         keep.append(y)
         x = y
-    if len(steps) > 8:
-        return _propagate_mean_post_unfused(A, ego, n_layers, post_csr, post_x, post_layers, post_row0)
-    arr = (_lib.SpmmStep * len(steps))(*steps)
-    rc = _lib.load().mmrec_spmm_chain_f32(d, len(steps), ctypes.cast(arr, ctypes.c_void_p), _stream())
+    if len(waves) > 8:
+        return unfused()
+    waves.sort(key=lambda w: (w[0], w[1]))                          # within a wave: the A_hat layer first, the shorter product fills its tail
+    steps = [_chain_step(M, sync_before=i > 0 and w != waves[i - 1][0], **kw) for i, (w, _, M, kw) in enumerate(waves)]
+    arr = (_lib.SpmmStep2 * len(steps))(*steps)
+    rc = _lib.load().mmrec_spmm_steps_f32(d, len(steps), ctypes.cast(arr, ctypes.c_void_p), int(cooperative), _stream())
     if rc == -4:                                                     # MMREC_EUNSUPPORTED: shape without a chained kernel
-        return _propagate_mean_post_unfused(A, ego, n_layers, post_csr, post_x, post_layers, post_row0)
-    check(rc, "mmrec_spmm_chain_f32")
+        return unfused()
+    check(rc, "mmrec_spmm_steps_f32")
     return acc
 
 
@@ -382,8 +407,6 @@ def propagate_mean(A: CSR, ego: torch.Tensor, n_layers: int) -> torch.Tensor:
     """mean(E_0 .. E_L), E_{l+1} = A E_l -- the LightGCN propagation every graph model repeats
     (`src/models/freedom.py:169-176`, `bm3.py:86-92`, `lightgcn.py:116-123`, `mgcn.py:159-166`), with the
     running sum and the final division fused into the SpMM epilogue (no stack, no extra passes)."""
-    if CHAIN and n_layers >= 1 and isinstance(A, CSR) and not (torch.is_grad_enabled() and ego.requires_grad):
-        return propagate_mean_fused(A, ego, n_layers)               # inference: all layers in one cooperative launch
     return _PropagateMeanFn.apply(ego, A, n_layers)
 
 
