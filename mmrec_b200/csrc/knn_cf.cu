@@ -10,8 +10,8 @@
 //   knn_norm_kernel     one warp per table row: largest |element| of the table (its bit pattern; inf / NaN patterns sort
 //                       above every finite one, so a non-finite element is detected here) and each row's norm, rounded up.
 //   knn_pack_kernel     X (and per row block the query rows) -> fp16, round to nearest, after ONE power-of-two scale sc for
-//                       the whole table that brings the largest element into [2^14, 2^15) (as cf_pack_kernel in
-//                       score_cf.cu), into the canonical K-major no-swizzle wgmma layout: tiles of 128 rows, K padded to a
+//                       the whole table that brings the largest element into [2^14, 2^15) (fp16_scale_for,
+//                       tc_common.cuh), into the canonical K-major no-swizzle wgmma layout: tiles of 128 rows, K padded to a
 //                       multiple of 64 with zeros; a 64-wide K chunk of a tile is one contiguous 16 KB range.
 //   knn_pass_kernel     s~ = the scaled score on the tensor cores (wgmma m64n128k16 f16 -> fp32), K-loop over F in chunks of
 //                       64 streamed through a 4-stage bulk-copy / mbarrier ring (48 KB per stage: 256 query rows + 128
@@ -53,6 +53,7 @@
 #include <cstdlib>
 
 #include "gemm_simt.cuh"
+#include "select.cuh"
 #include "tc_common.cuh"
 
 namespace mmrec {
@@ -103,13 +104,6 @@ __global__ void __launch_bounds__(256) knn_norm_kernel(int64_t n, const float* _
     if (lane == 0 && nmax) atomicMax(header + 1, nmax);               // (a NaN norm only happens with a non-finite element)
 }
 
-// 2^(14 - e) for the largest magnitude's exponent e (1 for zero / non-finite / tiny tables), as cf_scale_for in score_cf.cu
-__device__ __forceinline__ float knn_scale(uint32_t m_bits) {
-    const uint32_t e = (m_bits >> 23) & 0xffu;
-    if (e == 0u || e == 255u || e < 14u) return 1.0f;
-    return __uint_as_float((268u - e) << 23);
-}
-
 // One thread per (tile, k block of 8, row of the tile): consecutive threads write one contiguous 2 KB core-matrix column and
 // read one 32-byte sector each.  Source row = idx ? idx[row] : row_off + row; rows >= n_rows are zero.
 __global__ void __launch_bounds__(256) knn_pack_kernel(int64_t n_rows, const int64_t* __restrict__ idx, int64_t row_off,
@@ -123,7 +117,7 @@ __global__ void __launch_bounds__(256) knn_pack_kernel(int64_t n_rows, const int
     const int kb = (int)(tk % kblks);
     const int64_t tile = tk / kblks;
     const int64_t row = tile * KN_TILE + rr;
-    const float sc = knn_scale(__ldg(header));
+    const float sc = fp16_scale_for(__ldg(header));
     float x[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) x[e] = 0.f;
@@ -282,13 +276,12 @@ __global__ void __launch_bounds__(KN_THREADS, 1) knn_pass_kernel(const KnnParams
 }
 
 // ---- threshold ------------------------------------------------------------------------------------------------------
-// One CTA per row.  Radix select over the order-preserving keys of the row's group maxima, 8 bits per pass, top 24 bits:
-// the result is the lower edge of the bucket holding the k-th largest maximum, so at least k maxima are >= it.
+// One CTA per row.  Radix select (cta_radix_select, select.cuh) over the keys of the row's group maxima, top 24 bits: the
+// result is the lower edge of the bucket holding the k-th largest maximum, so at least k maxima are >= it.
 __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int64_t G_valid, int k, int F, const float* __restrict__ gmax,
                                                       const int64_t* __restrict__ rows, int64_t row_off, const float* __restrict__ rnorm,
                                                       const uint32_t* __restrict__ header, float* __restrict__ thr, int32_t* __restrict__ flags) {
-    __shared__ unsigned hist[256];
-    __shared__ unsigned s_prefix, s_need;
+    __shared__ RadixSmem sm;
     const int64_t row = blockIdx.x;
     const int tid = threadIdx.x;
     if (row >= nb) return;
@@ -297,34 +290,11 @@ __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int
         return;
     }
     const float* g = gmax + row * G;
-    unsigned prefix = 0, need = (unsigned)k;
-    for (int pass = 0; pass < 3; ++pass) {
-        const int shift = 24 - 8 * pass;
-        const unsigned hi_mask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-        hist[tid] = 0;
-        __syncthreads();
-        for (int64_t i = tid; i < G_valid; i += 256) {
-            const unsigned key = float_key(__ldg(g + i));
-            if ((key & hi_mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
-        }
-        __syncthreads();
-        if (tid == 0) {
-            unsigned cum = 0;
-            int dgt = 255;
-            for (; dgt > 0; --dgt) {
-                if (cum + hist[dgt] >= need) break;
-                cum += hist[dgt];
-            }
-            s_prefix = prefix | ((unsigned)dgt << shift);
-            s_need = need - cum;
-        }
-        __syncthreads();
-        prefix = s_prefix; need = s_need;
-        __syncthreads();
-    }
+    unsigned need = (unsigned)k;
+    const unsigned prefix = cta_radix_select<3, 256>([=](int64_t i) { return float_key(__ldg(g + i)); }, G_valid, need, sm);
     if (tid == 0) {
         const float t = key_float(prefix);
-        const float sc = knn_scale(header[0]);
+        const float sc = fp16_scale_for(header[0]);
         const int64_t qrow = rows ? rows[row] : row_off + row;
         const float un = rnorm[qrow] * sc, mn = __uint_as_float(header[1]) * sc;
         const float steps = (float)((F + KN_KC - 1) / KN_KC * (KN_KC / 16));
@@ -359,20 +329,6 @@ __device__ __forceinline__ float knn_exact(const float* __restrict__ q, const fl
     for (; k < F; ++k) acc = fmaf(__ldg(q + k), __ldg(x + k), acc);
     if (F & 31) acc = fmaf(0.f, 0.f, acc);
     return acc;
-}
-
-__device__ void knn_bitonic_desc(uint64_t* a, int n) {
-    for (int size = 2; size <= n; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            __syncthreads();
-            for (int t = threadIdx.x; t < n / 2; t += blockDim.x) {
-                const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-                const bool desc = ((lo & size) == 0);
-                const uint64_t x = a[lo], y = a[hi];
-                if ((x < y) == desc) { a[lo] = y; a[hi] = x; }
-            }
-        }
-    __syncthreads();
 }
 
 __global__ void __launch_bounds__(KN_FIN_THREADS) knn_final_kernel(int64_t nb, int64_t n, const float* __restrict__ X, int64_t ldx, int F, int k,
@@ -421,7 +377,7 @@ __global__ void __launch_bounds__(KN_FIN_THREADS) knn_final_kernel(int64_t nb, i
         }
         comp[c] = v;
     }
-    knn_bitonic_desc(comp, n2);
+    bitonic_desc(comp, n2);
     for (int t = tid; t < k; t += KN_FIN_THREADS) {
         const uint64_t c = comp[t];
         out_idx[row * k + t] = (int64_t)(uint32_t)(~(uint32_t)c);

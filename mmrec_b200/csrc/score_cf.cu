@@ -37,6 +37,7 @@
 #include <cstdlib>
 #include <cub/device/device_scan.cuh>
 
+#include "select.cuh"
 #include "tc_common.cuh"
 
 namespace mmrec {
@@ -255,14 +256,6 @@ __global__ void __launch_bounds__(CF_THREADS, 1) cf_pass_kernel(const CfParams p
 // ------------------------------------------------------------------------------------------------------------------
 // operand packing
 // ------------------------------------------------------------------------------------------------------------------
-// Power of two that brings a largest magnitude m into [2^14, 2^15) (m = 0, inf, NaN, or below 2^-113: 1 -- the
-// non-finite cases flag their rows in cf_thr_kernel; the tiny ones are what CF_EPS_SUB in the margin is for).
-__device__ __forceinline__ float cf_scale_for(uint32_t m_bits) {
-    const uint32_t e = (m_bits >> 23) & 0xffu;                       // biased exponent
-    if (e == 0u || e == 255u || e < 14u) return 1.0f;
-    return __uint_as_float((268u - e) << 23);                        // 2^(14 - (e - 127))
-}
-
 // One thread per (padded row, k block of 8): scale, round to fp16, store 16 bytes into the tile layout; the KP/8 threads
 // of a row are consecutive lanes and reduce the row's squared norm (and, for user rows, its largest magnitude) with
 // shuffles.  `scale_src` = the catalogue-wide largest magnitude (items), or NULL: per-row scale (users).
@@ -290,7 +283,7 @@ __device__ __forceinline__ void cf_pack_one(int64_t t, int64_t n_rows, const int
             am = a2 > am ? a2 : am;
         }
     }
-    const float sc = cf_scale_for(scale_src ? __ldg(scale_src) : am);
+    const float sc = fp16_scale_for(scale_src ? __ldg(scale_src) : am);
     // the norm is taken of the scaled row: squares of unscaled elements below ~1e-19 underflow to 0 (and above ~1e19
     // overflow), which would shrink the margin of cf_thr_kernel to its subnormal term while the operands are full size
     float ss = 0.f;
@@ -843,38 +836,20 @@ __global__ void __launch_bounds__(32 * CF_FIN_WARPS, LPR <= 16 ? 8 : 6) cf_final
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// exact fp32 rows (flagged only): all items on CUDA cores, mask, radix select, ordered ties, sort -- the contract of
-// mmrec_topk_rows_f32.  CTA `sl` serves the flagged rows sl, sl + CF_EX_SLOTS, ... with its own key buffer; all CTAs
-// exit at once when nothing was flagged.
+// exact fp32 rows (flagged only): all items on CUDA cores, mask, then the selection of mmrec_topk_rows_f32
+// (cta_topk_from_keys, select.cuh).  CTA `sl` serves the flagged rows sl, sl + CF_EX_SLOTS, ... with its own key buffer;
+// all CTAs exit at once when nothing was flagged.
 // ------------------------------------------------------------------------------------------------------------------
-__device__ void cf_bitonic_desc(uint64_t* a, int n) {
-    for (int size = 2; size <= n; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            __syncthreads();
-            for (int t = threadIdx.x; t < n / 2; t += blockDim.x) {
-                int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-                bool desc = ((lo & size) == 0);
-                uint64_t x = a[lo], y = a[hi];
-                if ((x < y) == desc) { a[lo] = y; a[hi] = x; }
-            }
-        }
-    __syncthreads();
-}
-
 __global__ void __launch_bounds__(256) cf_exact_kernel(const int64_t* __restrict__ users, const float* __restrict__ Ue, int64_t ldu,
                                                        int64_t n_items, const float* __restrict__ Ie, int64_t ldi, int d, int k,
                                                        int64_t item_offset, const int32_t* __restrict__ mask_ptr,
                                                        const int32_t* __restrict__ mask_items, const int32_t* __restrict__ counter,
                                                        const int32_t* __restrict__ row_of_slot, unsigned* __restrict__ keys_all,
                                                        int64_t* __restrict__ out_idx, float* __restrict__ out_val) {
-    __shared__ unsigned hist[256];
-    __shared__ uint64_t sel[1024];
-    __shared__ unsigned tie_idx[1024];
-    __shared__ unsigned s_prefix, s_need, s_count, s_base, n_ties;
-    __shared__ unsigned warp_tot[8];
+    __shared__ TopkSmem sm;
     __shared__ __align__(16) float u_ex[128];
     const int n_flagged = *counter;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int tid = threadIdx.x;
     unsigned* keys = keys_all + (int64_t)blockIdx.x * n_items;
     for (int fr = blockIdx.x; fr < n_flagged; fr += gridDim.x) {
         const int64_t row = row_of_slot[fr];
@@ -892,80 +867,7 @@ __global__ void __launch_bounds__(256) cf_exact_kernel(const int64_t* __restrict
             if (item >= 0 && item < n_items) keys[item] = float_key(-1e10f);          // src/common/trainer.py:307
         }
         __syncthreads();
-        // ---- radix select of the k-th largest key
-        unsigned prefix = 0, need = (unsigned)k;
-        for (int pass = 0; pass < 4; ++pass) {
-            const int shift = 24 - 8 * pass;
-            const unsigned hi_mask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-            hist[tid] = 0;
-            __syncthreads();
-            for (int64_t i = tid; i < n_items; i += 256) {
-                const unsigned key = keys[i];
-                if ((key & hi_mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
-            }
-            __syncthreads();
-            if (tid == 0) {
-                unsigned cum = 0;
-                int dgt = 255;
-                for (; dgt > 0; --dgt) {
-                    if (cum + hist[dgt] >= need) break;
-                    cum += hist[dgt];
-                }
-                s_prefix = prefix | ((unsigned)dgt << shift);
-                s_need = need - cum;
-            }
-            __syncthreads();
-            prefix = s_prefix; need = s_need;
-            __syncthreads();
-        }
-        const unsigned kth = prefix;
-        if (tid == 0) { s_count = 0; s_base = 0; n_ties = 0; }
-        __syncthreads();
-        const unsigned n_gt = (unsigned)k - need;
-        // strictly greater keys in any order; the indices of the keys equal to the k-th are collected and the `need` lowest
-        // of them taken (normally there is exactly one)
-        for (int64_t i = tid; i < n_items; i += 256) {
-            const unsigned key = keys[i];
-            if (key > kth) { unsigned pos = atomicAdd(&s_count, 1u); sel[pos] = ((uint64_t)key << 32) | (uint32_t)(~(uint32_t)i); }
-            else if (key == kth) { unsigned pos = atomicAdd(&n_ties, 1u); if (pos < 1024u) tie_idx[pos] = (unsigned)i; }
-        }
-        __syncthreads();
-        if (n_ties <= 1024u) {
-            const unsigned nt = n_ties;
-            for (unsigned t = tid; t < nt; t += 256) {
-                const unsigned me = tie_idx[t];
-                unsigned rank = 0;
-                for (unsigned u2 = 0; u2 < nt; ++u2) rank += tie_idx[u2] < me;
-                if (rank < need) sel[n_gt + rank] = ((uint64_t)kth << 32) | (uint32_t)(~me);
-            }
-        } else {
-            // degenerate row (thousands of equal scores): ordered sweep, 256 items at a time
-            for (int64_t i0 = 0; i0 < n_items; i0 += 256) {
-                const int64_t i = i0 + tid;
-                const bool eq = i < n_items && keys[i] == kth;
-                const unsigned bal = __ballot_sync(0xffffffffu, eq);
-                if (lane == 0) warp_tot[wid] = __popc(bal);
-                __syncthreads();
-                unsigned off = s_base;
-                for (int w = 0; w < wid; ++w) off += warp_tot[w];
-                const unsigned rank = off + __popc(bal & ((1u << lane) - 1u));
-                if (eq && rank < need) sel[n_gt + rank] = ((uint64_t)kth << 32) | (uint32_t)(~(uint32_t)i);
-                __syncthreads();
-                if (tid == 0) { unsigned tot = 0; for (int w = 0; w < 8; ++w) tot += warp_tot[w]; s_base += tot; }
-                __syncthreads();
-                if (s_base >= need) break;
-            }
-        }
-        __syncthreads();
-        int n2 = 1;
-        while (n2 < k) n2 <<= 1;
-        for (int t = k + tid; t < n2; t += 256) sel[t] = 0;
-        cf_bitonic_desc(sel, n2);
-        for (int t = tid; t < k; t += 256) {
-            const uint64_t c = sel[t];
-            out_idx[row * k + t] = (int64_t)(uint32_t)(~(uint32_t)c) + item_offset;
-            out_val[row * k + t] = key_float((uint32_t)(c >> 32));
-        }
+        cta_topk_from_keys<256>([=](int64_t i) { return keys[i]; }, n_items, k, item_offset, out_idx + row * k, out_val + row * k, sm);
     }
 }
 

@@ -107,6 +107,16 @@ __device__ __forceinline__ void split_tf32_trunc(float x, float& hi, float& lo) 
 
 }  // namespace tc
 
+// Power of two that brings a largest magnitude m (its fp32 bit pattern) into [2^14, 2^15) before the fp16 rounding of the
+// f16 tensor-core operands: no overflow, and fp16 subnormals only for elements 2^-28 below the largest.  1 for m = 0, inf,
+// NaN or below 2^-113 -- the callers route non-finite tables and rows elsewhere, and carry a subnormal term in their
+// error bounds for the tiny ones.
+__device__ __forceinline__ float fp16_scale_for(uint32_t m_bits) {
+    const uint32_t e = (m_bits >> 23) & 0xffu;                       // biased exponent
+    if (e == 0u || e == 255u || e < 14u) return 1.0f;
+    return __uint_as_float((268u - e) << 23);                        // 2^(14 - (e - 127))
+}
+
 // ---- tile geometry shared by the tensor-core kernels ---------------------------------------------------------
 constexpr int TC_M = 128;          // users per CTA tile: two consumer warpgroups of 64 rows
 constexpr int TC_N = 256;          // items per accumulator (128 fp32 registers per thread)

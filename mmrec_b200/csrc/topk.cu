@@ -2,12 +2,13 @@
 // Contract (stronger than torch.topk, which leaves tie order open): descending value, equal values in
 // ascending item index.  Replaces src/common/trainer.py:307-309.
 //
-// mmrec_topk_rows_f32: one CTA per row.  Radix select (4 passes x 8 bits over order-preserving keys) finds
-// the k-th largest key; everything above it is gathered unordered, the ties on the k-th key are taken in
-// index order (block-wide ordered compaction), then a bitonic sort on the composite (key, ~index) puts the
-// k winners in contract order.  (A warp-per-row streaming filter with bitonic compaction was measured 2.5x
-// slower at 7k items: the compaction sorts dominate.)
+// mmrec_topk_rows_f32: one CTA per row, cta_topk_from_keys (select.cuh): radix select (4 passes x 8 bits over
+// order-preserving keys) finds the k-th largest key; everything above it is gathered unordered, the ties on the
+// k-th key are taken in index order (block-wide ordered compaction), then a bitonic sort on the composite
+// (key, ~index) puts the k winners in contract order.  (A warp-per-row streaming filter with bitonic compaction
+// was measured 2.5x slower at 7k items: the compaction sorts dominate.)
 #include "peer_sync.cuh"
+#include "select.cuh"
 
 namespace mmrec {
 
@@ -19,107 +20,15 @@ __global__ void mask_kernel(int64_t nnz, const int64_t* __restrict__ rows, const
     if (r >= 0 && r < B && c >= 0 && c < n_items) S[r * ldS + c] = -1e10f;   // trainer.py:307
 }
 
-constexpr int TOPK_THREADS = 256;
-constexpr int TOPK_MAXK = 1024;
-
-// bitonic sort of n (power of two) 64-bit composites in shared memory, DESCENDING
-__device__ void bitonic_desc(uint64_t* a, int n) {
-    for (int size = 2; size <= n; size <<= 1) {
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            __syncthreads();
-            for (int t = threadIdx.x; t < n / 2; t += blockDim.x) {
-                int lo = 2 * t - (t & (stride - 1));
-                int hi = lo + stride;
-                bool desc = ((lo & size) == 0);
-                uint64_t x = a[lo], y = a[hi];
-                if ((x < y) == desc) { a[lo] = y; a[hi] = x; }
-            }
-        }
-    }
-    __syncthreads();
-}
+constexpr int TOPK_THREADS = SELECT_THREADS;
 
 __global__ void __launch_bounds__(TOPK_THREADS) topk_rows_kernel(int64_t n_items, const float* __restrict__ S, int64_t ldS,
                                                                  int k, int64_t item_offset, int64_t* __restrict__ out_idx,
                                                                  float* __restrict__ out_val) {
-    __shared__ unsigned hist[256];
-    __shared__ uint64_t sel[TOPK_MAXK];
-    __shared__ unsigned s_prefix, s_need, s_count, s_base;
-    __shared__ unsigned warp_tot[TOPK_THREADS / 32];
+    __shared__ TopkSmem sm;
     const float* row = S + (int64_t)blockIdx.x * ldS;
-    const int tid = threadIdx.x;
-
-    // ---- radix select: after the loop `prefix` is the key of the k-th largest element, `need` the number
-    //      of elements equal to it that belong to the top-k
-    unsigned prefix = 0, need = (unsigned)k;
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 24 - 8 * pass;
-        const unsigned hi_mask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-        hist[tid] = 0;
-        __syncthreads();
-        for (int64_t i = tid; i < n_items; i += TOPK_THREADS) {
-            unsigned key = float_key(row[i]);
-            if ((key & hi_mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
-        }
-        __syncthreads();
-        if (tid == 0) {
-            unsigned cum = 0;
-            int dgt = 255;
-            for (; dgt > 0; --dgt) {
-                if (cum + hist[dgt] >= need) break;
-                cum += hist[dgt];
-            }
-            s_prefix = prefix | ((unsigned)dgt << shift);
-            s_need = need - cum;
-        }
-        __syncthreads();
-        prefix = s_prefix; need = s_need;
-        __syncthreads();
-    }
-    const unsigned kth = prefix;
-    // ---- gather: strictly greater (any order), then ties in index order
-    if (tid == 0) { s_count = 0; s_base = 0; }
-    __syncthreads();
-    for (int64_t i = tid; i < n_items; i += TOPK_THREADS) {
-        unsigned key = float_key(row[i]);
-        if (key > kth) {
-            unsigned p = atomicAdd(&s_count, 1u);
-            sel[p] = ((uint64_t)key << 32) | (uint32_t)(~(uint32_t)i);
-        }
-    }
-    __syncthreads();
-    const unsigned n_gt = s_count;     // == k - need
-    for (int64_t i0 = 0; i0 < n_items; i0 += TOPK_THREADS) {
-        if (s_base >= need) break;
-        const int64_t i = i0 + tid;
-        const bool eq = i < n_items && float_key(row[i]) == kth;
-        const unsigned bal = __ballot_sync(0xffffffffu, eq);
-        const int lane = tid & 31, wid = tid >> 5;
-        if (lane == 0) warp_tot[wid] = __popc(bal);
-        __syncthreads();
-        unsigned off = s_base;
-        for (int w = 0; w < wid; ++w) off += warp_tot[w];
-        const unsigned rank = off + __popc(bal & ((1u << lane) - 1u));
-        if (eq && rank < need) sel[n_gt + rank] = ((uint64_t)kth << 32) | (uint32_t)(~(uint32_t)i);
-        __syncthreads();
-        if (tid == 0) {
-            unsigned tot = 0;
-            for (int w = 0; w < TOPK_THREADS / 32; ++w) tot += warp_tot[w];
-            s_base += tot;
-        }
-        __syncthreads();
-    }
-    // ---- order the k winners
-    int n2 = 1;
-    while (n2 < k) n2 <<= 1;
-    for (int t = k + tid; t < n2; t += TOPK_THREADS) sel[t] = 0;   // pads sort last (key 0 < any real key)
-    __syncthreads();
-    bitonic_desc(sel, n2);
-    for (int t = tid; t < k; t += TOPK_THREADS) {
-        uint64_t c = sel[t];
-        out_idx[(int64_t)blockIdx.x * k + t] = (int64_t)(uint32_t)(~(uint32_t)c) + item_offset;
-        out_val[(int64_t)blockIdx.x * k + t] = key_float((uint32_t)(c >> 32));
-    }
+    cta_topk_from_keys<TOPK_THREADS>([=](int64_t i) { return float_key(row[i]); }, n_items, k, item_offset,
+                                     out_idx + (int64_t)blockIdx.x * k, out_val + (int64_t)blockIdx.x * k, sm);
 }
 
 // merge `parts` sorted [B,k] lists per row.  Candidates parts*k <= 4096.
