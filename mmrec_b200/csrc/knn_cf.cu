@@ -7,19 +7,21 @@
 // zeros to a multiple of 32 (a padding step fmaf(0, 0, acc) turns a -0.0 sum into +0.0), ranked on float_key (common.cuh).
 // Every value this file returns is that chain (knn_exact below), and the order is taken on those values.
 //
-//   knn_norm_kernel     one warp per table row: largest |element| of the table (its bit pattern; inf / NaN patterns sort
+//   absmax_norm_kernel  one warp per table row: largest |element| of the table (its bit pattern; inf / NaN patterns sort
 //                       above every finite one, so a non-finite element is detected here) and each row's norm, rounded up.
 //   knn_pack_kernel     X (and per row block the query rows) -> fp16, round to nearest, after ONE power-of-two scale sc for
 //                       the whole table that brings the largest element into [2^14, 2^15) (fp16_scale_for,
-//                       tc_common.cuh), into the canonical K-major no-swizzle wgmma layout: tiles of 128 rows, K padded to a
-//                       multiple of 64 with zeros; a 64-wide K chunk of a tile is one contiguous 16 KB range.
+//                       tc_common.cuh), into the canonical K-major no-swizzle wgmma layout (store_fp16x8): tiles of 128
+//                       rows, K padded to a multiple of 64 with zeros; a 64-wide K chunk of a tile is one contiguous 16 KB
+//                       range.
 //   knn_pass_kernel     s~ = the scaled score on the tensor cores (wgmma m64n128k16 f16 -> fp32), K-loop over F in chunks of
 //                       64 streamed through a 4-stage bulk-copy / mbarrier ring (48 KB per stage: 256 query rows + 128
-//                       items).  Epilogue: the maximum of every group of 16 consecutive items, gmax[row][group].  A unit =
-//                       (pair of 128-row query tiles, 128-item tile); units are dealt to the CTAs in contiguous runs, the
-//                       query pair varies fastest so that consecutive units reuse the item tile from L2.
+//                       items).  Epilogue (group_max_store<8>): the maximum of every group of 16 consecutive items,
+//                       gmax[row][group].  A unit = (pair of 128-row query tiles, 128-item tile); units are dealt to the
+//                       CTAs in contiguous runs, the query pair varies fastest so that consecutive units reuse the item
+//                       tile from L2.
 //   knn_thr_kernel      one CTA per row: t = a value <= the k-th largest group maximum with at least k maxima >= t (radix
-//                       select on the top 24 key bits, lower bucket edge); thr = t - 2 eps'.
+//                       select on the top 24 key bits, lower bucket edge); thr = t - 2 eps' (set_threshold).
 //   knn_final_kernel    one CTA per row: every group with gmax >= thr -> every item of those groups scored EXACTLY (knn_exact,
 //                       from the original fp32 rows) -> bitonic sort on (float_key, ~index) -> top-k.
 //   exact route         rows the filter does not serve (fewer than k groups, more than KN_CAP candidates, a non-finite
@@ -73,10 +75,9 @@ constexpr int KN_GROUP = 16;                            // items per group maxim
 constexpr int KN_CAP = 4096;                            // candidates (16 x surviving groups) one CTA scores per row
 constexpr int KN_FIN_THREADS = 256;
 
-// ---- table norms / largest magnitude ------------------------------------------------------------------------------
-// header words: [0] largest |element| bits, [1] largest row norm bits (unscaled, rounded up); zeroed before the launch
-__global__ void __launch_bounds__(256) knn_norm_kernel(int64_t n, const float* __restrict__ X, int64_t ldx, int F,
-                                                       float* __restrict__ rnorm, uint32_t* __restrict__ header) {
+// ---- table norms / largest magnitude (declared in tc_common.cuh; score_cf.cu runs it without the norms) -------------
+__global__ void __launch_bounds__(256) absmax_norm_kernel(int64_t n, const float* __restrict__ X, int64_t ldx, int F, float* __restrict__ rnorm,
+                                                          uint32_t* __restrict__ amax_out, uint32_t* __restrict__ nmax_out) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = (int64_t)gridDim.x * 8;
     // a per-lane chain of ceil(F / 32) squares and a 5-level tree: relative error of the sum of squares below (F/32 + 6) 2^-24
@@ -85,23 +86,23 @@ __global__ void __launch_bounds__(256) knn_norm_kernel(int64_t n, const float* _
     for (int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n; r += warps) {
         const float* row = X + r * ldx;
         float ss = 0.f;
-        uint32_t am = 0u;
         for (int c = lane; c < F; c += 32) {
             const float x = __ldg(row + c);
             ss = fmaf(x, x, ss);
             const uint32_t b = __float_as_uint(x) & 0x7fffffffu;
-            am = b > am ? b : am;
+            amax = b > amax ? b : amax;
         }
-        ss = warp_sum(ss);
-        am = __reduce_max_sync(0xffffffffu, am);
-        const float nrm = sqrtf(ss) * up;
-        if (lane == 0) rnorm[r] = nrm;
-        amax = am > amax ? am : amax;
-        const uint32_t nb = __float_as_uint(nrm);
-        nmax = nb > nmax ? nb : nmax;
+        if (rnorm) {
+            ss = warp_sum(ss);
+            const float nrm = sqrtf(ss) * up;
+            if (lane == 0) rnorm[r] = nrm;
+            const uint32_t nb = __float_as_uint(nrm);
+            nmax = nb > nmax ? nb : nmax;
+        }
     }
-    if (lane == 0 && amax) atomicMax(header + 0, amax);
-    if (lane == 0 && nmax) atomicMax(header + 1, nmax);               // (a NaN norm only happens with a non-finite element)
+    amax = __reduce_max_sync(0xffffffffu, amax);
+    if (lane == 0 && amax) atomicMax(amax_out, amax);
+    if (lane == 0 && nmax) atomicMax(nmax_out, nmax);                // (a NaN norm only happens with a non-finite element)
 }
 
 // One thread per (tile, k block of 8, row of the tile): consecutive threads write one contiguous 2 KB core-matrix column and
@@ -132,13 +133,7 @@ __global__ void __launch_bounds__(256) knn_pack_kernel(int64_t n_rows, const int
                 if (kb * 8 + e < F) x[e] = __ldg(src + e);
         }
     }
-    uint32_t w[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const __half2 h = __floats2half2_rn(x[2 * e] * sc, x[2 * e + 1] * sc);
-        w[e] = *reinterpret_cast<const uint32_t*>(&h);
-    }
-    out[((tile * kblks + kb) * (KN_TILE / 8) + rr / 8) * 8 + (rr % 8)] = make_uint4(w[0], w[1], w[2], w[3]);
+    store_fp16x8(out, tile, kblks, kb, rr, x, sc);
 }
 
 // ---- the tensor-core pass ---------------------------------------------------------------------------------------------
@@ -169,31 +164,6 @@ __device__ __forceinline__ void knn_producer(const KnnParams& p, uint32_t sbase,
             bulk_g2s(dst + KN_CHUNK, a0 + tile_bytes + off, KN_CHUNK, full);
             bulk_g2s(dst + 2 * KN_CHUNK, b0 + off, KN_CHUNK, full);
             if (++slot == KN_STAGES) { slot = 0; ph ^= 1; }
-        }
-    }
-}
-
-// rows row0 and row0 + 8 of one m64 accumulator (fragment layout: wgmma.cuh); lane q of a quad stores groups g = q, q + 4
-__device__ __forceinline__ void knn_group_max(const float (&acc)[64], int row0, int n_valid, int q, int it, const KnnParams& p) {
-#pragma unroll
-    for (int e2 = 0; e2 < 2; ++e2) {
-        const int row = row0 + 8 * e2;
-        float gm[8];
-#pragma unroll
-        for (int g = 0; g < 8; ++g) {
-            float m = -INFINITY;
-#pragma unroll
-            for (int j = 2 * g; j < 2 * g + 2; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e)
-                    if (8 * j + 2 * q + e < n_valid) m = fmaxf(m, acc[4 * j + 2 * e2 + e]);
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-            gm[g] = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-        }
-        if (row < p.nb) {
-            float* dst = p.gmax + (row * p.G + it * 8);      // (< 2^27: a row block's maxima stay below 512 MB)
-            dst[q] = q == 0 ? gm[0] : (q == 1 ? gm[1] : (q == 2 ? gm[2] : gm[3]));
-            dst[q + 4] = q == 0 ? gm[4] : (q == 1 ? gm[5] : (q == 2 ? gm[6] : gm[7]));
         }
     }
 }
@@ -242,11 +212,15 @@ __device__ __forceinline__ void knn_consumer(const KnnParams& p, uint32_t sbase,
         wgmma_fence_regs(acc0);
         wgmma_fence_regs(acc1);
         warp_arrive(bar + (KN_STAGES + prev) * 8);
-        // ---- epilogue: maxima of the 8 groups of 16 columns; columns >= n_valid (last item tile) read as -inf
+        // ---- epilogue: maxima of the 8 groups of 16 columns of rows row0 + 8 e2 (acc0) and row0 + 64 + 8 e2 (acc1)
         const int n_valid = p.n - cur_it * KN_TILE;
         const int row0 = base + 16 * w + (lane >> 2);
-        knn_group_max(acc0, row0, n_valid, q, cur_it, p);
-        knn_group_max(acc1, row0 + 64, n_valid, q, cur_it, p);
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int row = row0 + 64 * (r >> 1) + 8 * (r & 1);
+            // (row * G < 2^27: a row block's maxima stay below 512 MB)
+            group_max_store<8>(r < 2 ? acc0 : acc1, r & 1, q, n_valid, row, p.nb, [&] { return p.gmax + (row * p.G + cur_it * 8); });
+        }
     }
 }
 
@@ -276,7 +250,7 @@ __global__ void __launch_bounds__(KN_THREADS, 1) knn_pass_kernel(const KnnParams
 }
 
 // ---- threshold ------------------------------------------------------------------------------------------------------
-// One CTA per row.  Radix select (cta_radix_select, select.cuh) over the keys of the row's group maxima, top 24 bits: the
+// One CTA per row.  Radix select (radix_select, select.cuh) over the keys of the row's group maxima, top 24 bits: the
 // result is the lower edge of the bucket holding the k-th largest maximum, so at least k maxima are >= it.
 __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int64_t G_valid, int k, int F, const float* __restrict__ gmax,
                                                       const int64_t* __restrict__ rows, int64_t row_off, const float* __restrict__ rnorm,
@@ -291,18 +265,15 @@ __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int
     }
     const float* g = gmax + row * G;
     unsigned need = (unsigned)k;
-    const unsigned prefix = cta_radix_select<3, 256>([=](int64_t i) { return float_key(__ldg(g + i)); }, G_valid, need, sm);
+    const unsigned prefix = radix_select<3, 256>([=](int64_t i) { return float_key(__ldg(g + i)); }, G_valid, need, sm);
     if (tid == 0) {
-        const float t = key_float(prefix);
         const float sc = fp16_scale_for(header[0]);
         const int64_t qrow = rows ? rows[row] : row_off + row;
         const float un = rnorm[qrow] * sc, mn = __uint_as_float(header[1]) * sc;
         const float steps = (float)((F + KN_KC - 1) / KN_KC * (KN_KC / 16));
         const float eps = 0x1p-10f + 0x1p-22f + (steps * 0x1p-22f + (float)F * 0x1p-24f) * (1.0f + 0x1p-9f);
         const float sub = 0x1p-25f * sqrtf((float)F) * (un + mn) + (float)F * 0x1p-50f + ((float)F * 0x1p-75f * sc) * (0x1p-74f * sc);
-        const float margin = 2.0f * (eps * un * mn + sub) * (1.0f + 0x1p-8f);
-        if (!(fabsf(t) < INFINITY) || !(margin < INFINITY)) { thr[row] = INFINITY; flags[row] = 2; }
-        else { thr[row] = t - margin; flags[row] = 0; }
+        set_threshold(key_float(prefix), 2.0f * (eps * un * mn + sub) * (1.0f + 0x1p-8f), thr + row, flags + row);
     }
 }
 
@@ -512,11 +483,12 @@ extern "C" int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F,
     int32_t* counter = (int32_t*)(base + P.off_cnt);
     int64_t* fb_rows = (int64_t*)(base + P.off_fbr);
     int64_t* fb_pos = (int64_t*)(base + P.off_fbp);
-    // 1. norms + largest magnitude; a non-finite element sends the whole call to the exact route
+    // 1. norms + largest magnitude; a non-finite element sends the whole call to the exact route.  Header words: [0] largest
+    //    |element| bits, [1] largest row norm bits (unscaled, rounded up)
     MMREC_CUDA(cudaMemsetAsync(header, 0, 1024, stream));
     {
         const int64_t blocks = (n + 7) / 8;
-        knn_norm_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, stream>>>(n, X, ldx, F, rnorm, header);
+        absmax_norm_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, stream>>>(n, X, ldx, F, rnorm, header, header + 1);
         MMREC_LAUNCH_CHECK();
     }
     uint32_t h_amax = 0;

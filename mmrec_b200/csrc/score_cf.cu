@@ -14,12 +14,14 @@
 //                       largest element lands in [2^14, 2^15): no overflow, and fp16 subnormals only for elements
 //                       2^-28 below the largest.  Scores, norms and thresholds of a row all live in that scaled domain
 //                       (the exact re-scoring reads the original tables).  Row norms (users) / maximum row norm
-//                       (catalogue).  The catalogue side is packed once per embedding table (mmrec_catalog_pack_f32).
+//                       (catalogue).  The catalogue side is packed once per embedding table (mmrec_catalog_pack_f32), its
+//                       scale from the table's largest magnitude (absmax_norm_kernel, knn_cf.cu).
 //   cf_pass_kernel<1>   s~ for every (user, item); epilogue = maximum of every group of w = 16 gw consecutive items
-//                       (accumulator registers -> max tree -> quad shuffles), written as gmax[row][group].  No atomics.
+//                       (accumulator registers -> max tree -> quad shuffles: group_max_store), written as gmax[row][group].
+//                       No atomics.
 //   cf_thr_kernel       per row: t = the need-th largest group maximum, need = k + (masked items of the row).  At
 //                       least `need` distinct items have s~ >= t, so >= k unmasked ones have s >= t - eps'; hence every
-//                       member of the true top-k has s~ >= thr = t - 2 eps'.
+//                       member of the true top-k has s~ >= thr = t - 2 eps' (set_threshold).
 //   cf_pass_kernel<2>   s~ again (same instructions, same bits); epilogue = one bit per score, s~ >= thr, 128 bits per
 //                       (row, item tile) written as one 16-byte store.  ~ (need + a few) bits per row are set.
 //   cf_final_kernel     per row (one warp): the set bits -> drop masked items -> exact fp32 score from the ORIGINAL
@@ -191,22 +193,7 @@ __device__ __forceinline__ void cf_consumer(const CfParams& p, const CfSmem& L, 
                 return 8 * j + 2 * q + e < n_valid ? v : -INFINITY;
             };
             if (PASS == 1) {
-                // group of 16 columns = j = 2 g, 2 g + 1: this lane's 4 values, then the quad's maximum; wider groups fold
-                float gm[GPT];
-#pragma unroll
-                for (int g = 0; g < GPT; ++g) {
-                    float m = -INFINITY;
-#pragma unroll
-                    for (int j = g * (16 / GPT); j < (g + 1) * (16 / GPT); ++j) m = fmaxf(m, fmaxf(val(j, 0), val(j, 1)));
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-                    gm[g] = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-                }
-                if (row < p.B) {
-                    float* dst = p.gmax + row * p.G + (int64_t)cur_it * GPT;
-#pragma unroll
-                    for (int g = 0; g < GPT; ++g)
-                        if ((g & 3) == q) dst[g] = gm[g];
-                }
+                group_max_store<GPT>(r < 2 ? acc0 : acc1, e2, q, n_valid, row, p.B, [&] { return p.gmax + row * p.G + (int64_t)cur_it * GPT; });
             } else {
                 // bit (31 - c) of word b: column 32 b + c passes, s~ >= thr (the sign of the exact difference)
                 uint32_t wd[4] = {0u, 0u, 0u, 0u};
@@ -288,38 +275,14 @@ __device__ __forceinline__ void cf_pack_one(int64_t t, int64_t n_rows, const int
     // overflow), which would shrink the margin of cf_thr_kernel to its subnormal term while the operands are full size
     float ss = 0.f;
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { x[e] *= sc; ss = fmaf(x[e], x[e], ss); }       // (exact: a power of two, no overflow)
+    for (int e = 0; e < 8; ++e) ss = fmaf(x[e] * sc, x[e] * sc, ss);              // (exact: a power of two, no overflow)
     for (int o = kblks / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    uint32_t w[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const __half2 h = __floats2half2_rn(x[2 * e], x[2 * e + 1]);
-        w[e] = *reinterpret_cast<const uint32_t*>(&h);
-    }
-    const int64_t tile = row / CF_TILE;
-    const int rr = (int)(row % CF_TILE);
-    out[((tile * kblks + kb) * (CF_TILE / 8) + rr / 8) * 8 + (rr % 8)] = make_uint4(w[0], w[1], w[2], w[3]);
+    store_fp16x8(out, row / CF_TILE, kblks, kb, (int)(row % CF_TILE), x, sc);
     if (kb == 0 && row < n_rows) {
         const float nrm = sqrtf(ss) * (1.0f + 1e-6f);                 // norm of the scaled row (rounded up: the bound must hold)
         if (row_norm) row_norm[row] = nrm;
         if (max_norm) atomicMax(max_norm, __float_as_uint(nrm));      // non-negative floats order like their bit patterns
     }
-}
-
-// header: word 0 = running maximum (scaled) norm, word 4 = largest magnitude of the table, both zeroed by a memset node
-// before the launches; thread 0 of the pack kernel fills in the rest
-__global__ void __launch_bounds__(256) cf_item_absmax_kernel(int64_t n_items, const float* __restrict__ Ie, int64_t ldi, int d,
-                                                             uint32_t* __restrict__ header) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps = (int64_t)gridDim.x * 8;
-    uint32_t m = 0;
-    for (int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n_items; r += warps)        // warp per row
-        for (int c = lane; c < d; c += 32) {
-            const uint32_t b = __float_as_uint(__ldg(Ie + r * ldi + c)) & 0x7fffffffu;             // |x|; NaN patterns sort above inf
-            m = b > m ? b : m;
-        }
-    m = __reduce_max_sync(0xffffffffu, m);
-    if (lane == 0 && m) atomicMax(header + 4, m);
 }
 
 __global__ void __launch_bounds__(256) cf_pack_items_kernel(int64_t n_items, const float* __restrict__ Ie, int64_t ldi, int d, int KP,
@@ -473,53 +436,9 @@ __global__ void __launch_bounds__(256) cf_prep_kernel(int64_t mask_blocks, int64
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// threshold: the need-th largest group maximum of the row, minus the certified margin.  One warp per row.
+// threshold: the need-th largest group maximum of the row, minus the certified margin.  One warp per row: up to 1024
+// groups the register search below, beyond that the warp's radix select (radix_select, select.cuh).
 // ------------------------------------------------------------------------------------------------------------------
-// Warp radix select over 32-bit keys read through `key_at(t)`, t < n: returns the key of the `need`-th largest.
-template <typename F>
-__device__ __forceinline__ uint32_t cf_warp_kth(F key_at, int n, int need, uint32_t* hist, int lane) {
-    uint32_t prefix = 0;
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 24 - 8 * pass;
-        const uint32_t hi_mask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-        for (int b = lane; b < 256; b += 32) hist[b] = 0;
-        __syncwarp();
-        for (int t = lane; t < n; t += 32) {
-            const uint32_t key = key_at(t);
-            if ((key & hi_mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
-        }
-        __syncwarp();
-        // lane l owns bins [8l, 8l+8); `cum` = keys in the bins above (exclusive suffix sum)
-        uint32_t mine[8], tot = 0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { mine[j] = hist[lane * 8 + j]; tot += mine[j]; }
-        uint32_t incl = tot;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t v = __shfl_down_sync(0xffffffffu, incl, o);
-            if (lane + o < 32) incl += v;
-        }
-        uint32_t cum = incl - tot;
-        int dgt = -1;
-#pragma unroll
-        for (int j = 7; j >= 0; --j) {
-            if (dgt < 0) {
-                if (cum + mine[j] >= (uint32_t)need) dgt = lane * 8 + j;
-                else cum += mine[j];
-            }
-        }
-        const unsigned found = __ballot_sync(0xffffffffu, dgt >= 0);   // (never empty: need <= n)
-        const int win = found ? 31 - __clz(found) : 0;
-        dgt = __shfl_sync(0xffffffffu, dgt, win);
-        cum = __shfl_sync(0xffffffffu, cum, win);
-        if (dgt < 0) dgt = 0;
-        prefix |= (uint32_t)dgt << shift;
-        need -= (int)cum;
-        __syncwarp();
-    }
-    return prefix;
-}
-
 // The threshold does not have to be the exact need-th largest group maximum -- any value with at least `need` maxima at
 // or above it is certified.  So the search runs on the top CF_THR_BITS bits of the order-preserving key only (bit by
 // bit, counts by REDUX: no atomics, the values stay in registers) and takes the lower edge of that bucket: 16 bits =
@@ -559,7 +478,7 @@ __device__ __forceinline__ uint32_t cf_warp_kth_coarse(const float* __restrict__
 __global__ void __launch_bounds__(256) cf_thr_kernel(int64_t nb, int G, int G_valid, int k, int d, const float* __restrict__ gmax, const float* __restrict__ unorm,
                                                      const uint32_t* __restrict__ max_norm, const int32_t* __restrict__ mask_ptr,
                                                      float* __restrict__ thr, int32_t* __restrict__ flags) {
-    __shared__ uint32_t hist_all[8][256];
+    __shared__ RadixSmem radix_all[8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t row = (int64_t)blockIdx.x * 8 + warp;
     if (row >= nb) return;
@@ -572,17 +491,16 @@ __global__ void __launch_bounds__(256) cf_thr_kernel(int64_t nb, int G, int G_va
     uint32_t kth;
     if (G <= 16 * 32) kth = cf_warp_kth_coarse<16>(g, G, need, lane);
     else if (G <= 32 * 32) kth = cf_warp_kth_coarse<32>(g, G, need, lane);
-    else kth = cf_warp_kth([&](int t) { return float_key(__ldg(g + t)); }, G, need, hist_all[warp], lane);
+    else {
+        unsigned need_u = (unsigned)need;
+        kth = radix_select<4, 32>([=](int64_t t) { return float_key(__ldg(g + t)); }, G, need_u, radix_all[warp]);
+    }
     if (lane == 0) {
-        const float t = key_float(kth);
         // scaled domain.  Per element |dx| <= 2^-11 |x| + 2^-25 (fp16 subnormals), so
         //   |s~ - s| <= 2^-10 |u| |i| (1 + 2^-12) + 2^-25 sqrt(d) (|u| + |i|) + (2^-25)^2 d + accumulation  <=  eps' below;
         // with the largest elements scaled into [2^14, 2^15) the second term is ~2^-38 of the first
         const float un = unorm[row], mn = __uint_as_float(*max_norm);
-        const float margin = 2.0f * (CF_EPS * un * mn + CF_EPS_SUB * sqrtf((float)d) * (un + mn + 1.0f));
-        const float out = t - margin;
-        if (!(fabsf(t) < INFINITY) || !(margin < INFINITY)) { thr[row] = INFINITY; flags[row] = 2; }   // NaN / inf scores
-        else thr[row] = out;
+        set_threshold(key_float(kth), 2.0f * (CF_EPS * un * mn + CF_EPS_SUB * sqrtf((float)d) * (un + mn + 1.0f)), thr + row, flags + row);
     }
 }
 
@@ -890,10 +808,12 @@ int cf_catalog_pack(int64_t n_items, const float* Ie, int64_t ldi, int d, void* 
     if (!need || !cat || cat_bytes < need || (((uintptr_t)cat) & 1023)) { set_error("catalog_pack: bad shape, or buffer null / not 1024-byte aligned / smaller than mmrec_catalog_bytes"); return MMREC_EINVAL; }
     const int KP = cf_kp(d);
     const int64_t n_it = (n_items + CF_TILE - 1) / CF_TILE;
+    // header: word 0 = running maximum (scaled) norm, word 4 = largest magnitude of the table, both zeroed here; thread 0
+    // of the pack kernel fills in the rest
     MMREC_CUDA(cudaMemsetAsync(cat, 0, CF_CAT_HEADER, stream));
     {
         const int64_t blocks = (n_items + 7) / 8;
-        cf_item_absmax_kernel<<<(unsigned)(blocks < 2368 ? blocks : 2368), 256, 0, stream>>>(n_items, Ie, ldi, d, (uint32_t*)cat);
+        absmax_norm_kernel<<<(unsigned)(blocks < 2368 ? blocks : 2368), 256, 0, stream>>>(n_items, Ie, ldi, d, nullptr, (uint32_t*)cat + 4, nullptr);
         MMREC_LAUNCH_CHECK();
     }
     const int64_t threads = n_it * CF_TILE * (KP / 8);

@@ -1,13 +1,13 @@
 // CTA-wide top-k selection over order-preserving 32-bit keys (float_key, common.cuh), shared by topk_rows_kernel
 // (topk.cu), cf_exact_kernel (score_cf.cu) and the kNN threshold / finalist kernels (knn_cf.cu), so that every one of
 // them returns the same order: values descending, equal values by ascending item index -- the composite
-// (key << 32 | ~index) sorted descending.
+// (key << 32 | ~index) sorted descending.  Its radix select also runs warp by warp (cf_thr_kernel, score_cf.cu).
 #pragma once
 #include "common.cuh"
 
 namespace mmrec {
 
-constexpr int SELECT_THREADS = 256;     // the radix select's histogram has one bin per thread
+constexpr int SELECT_THREADS = 256;     // threads of a CTA that selects
 constexpr int TOPK_MAXK = 1024;         // winners one CTA orders in shared memory
 
 // bitonic sort of n (power of two) 64-bit composites in shared memory, DESCENDING
@@ -39,38 +39,60 @@ struct TopkSmem {
     unsigned warp_tot[SELECT_THREADS / 32];
 };
 
-// Radix select over the keys key_at(0 .. n-1), 8 bits per pass from the top.  On entry `need` is the rank wanted (k);
-// on return the result is the top 8 * PASSES bits of the k-th largest key (the rest zero: with PASSES < 4, the lower edge of
-// its bucket, so at least k keys are >= it) and `need` the number of keys in that bucket that belong to the top k.
+// Radix select over the keys key_at(0 .. n-1), 8 bits per pass from the top, by a group of THREADS threads: one warp
+// (THREADS = 32, each warp of the CTA with its own `sm`) or the whole CTA (THREADS = SELECT_THREADS = blockDim.x).  On entry
+// `need` is the rank wanted (k); on return the result is the top 8 * PASSES bits of the k-th largest key (the rest zero:
+// with PASSES < 4, the lower edge of its bucket, so at least k keys are >= it) and `need` the number of keys in that bucket
+// that belong to the top k.  Per pass, the group counts the next digit of the keys under the prefix into `sm.hist`, then
+// the first warp finds the digit: lane l owns bins 8l .. 8l + 7, a suffix sum over the lanes gives the count above them,
+// and the highest lane whose bins reach `need` has the digit.
 template <int PASSES, int THREADS, class KeyAt>
-__device__ __forceinline__ unsigned cta_radix_select(KeyAt key_at, int64_t n, unsigned& need, RadixSmem& sm) {
-    static_assert(THREADS == SELECT_THREADS, "cta_radix_select: one histogram bin per thread, 256 threads");
-    static_assert(PASSES >= 1 && PASSES <= 4, "cta_radix_select: 1 to 4 passes of 8 bits");
-    const int tid = threadIdx.x;
+__device__ __forceinline__ unsigned radix_select(KeyAt key_at, int64_t n, unsigned& need, RadixSmem& sm) {
+    static_assert(THREADS == 32 || THREADS == SELECT_THREADS, "radix_select: one warp or the 256-thread CTA");
+    static_assert(PASSES >= 1 && PASSES <= 4, "radix_select: 1 to 4 passes of 8 bits");
+    const int tid = THREADS == 32 ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
+    auto group_sync = [] { if (THREADS == 32) __syncwarp(); else __syncthreads(); };
     unsigned prefix = 0;
     for (int pass = 0; pass < PASSES; ++pass) {
         const int shift = 24 - 8 * pass;
         const unsigned hi_mask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-        sm.hist[tid] = 0;
-        __syncthreads();
+        for (int b = tid; b < 256; b += THREADS) sm.hist[b] = 0;
+        group_sync();
         for (int64_t i = tid; i < n; i += THREADS) {
             unsigned key = key_at(i);
             if ((key & hi_mask) == prefix) atomicAdd(&sm.hist[(key >> shift) & 255u], 1u);
         }
-        __syncthreads();
-        if (tid == 0) {
-            unsigned cum = 0;
-            int dgt = 255;
-            for (; dgt > 0; --dgt) {
-                if (cum + sm.hist[dgt] >= need) break;
-                cum += sm.hist[dgt];
+        group_sync();
+        if (tid < 32) {
+            unsigned mine[8], tot = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { mine[j] = sm.hist[tid * 8 + j]; tot += mine[j]; }
+            unsigned incl = tot;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned v = __shfl_down_sync(0xffffffffu, incl, o);
+                if (tid + o < 32) incl += v;
             }
-            sm.prefix = prefix | ((unsigned)dgt << shift);
-            sm.need = need - cum;
+            unsigned cum = incl - tot;
+            int dgt = -1;
+#pragma unroll
+            for (int j = 7; j >= 0; --j) {
+                if (dgt < 0) {
+                    if (cum + mine[j] >= need) dgt = tid * 8 + j;
+                    else cum += mine[j];
+                }
+            }
+            const unsigned found = __ballot_sync(0xffffffffu, dgt >= 0);     // (never empty: need <= keys under the prefix)
+            const int win = found ? 31 - __clz(found) : 0;
+            dgt = __shfl_sync(0xffffffffu, dgt, win);
+            cum = __shfl_sync(0xffffffffu, cum, win);
+            if (tid == 0) {
+                sm.prefix = prefix | ((unsigned)(dgt < 0 ? 0 : dgt) << shift);
+                sm.need = need - cum;
+            }
         }
-        __syncthreads();
-        prefix = sm.prefix; need = sm.need;
-        __syncthreads();
+        group_sync();
+        prefix = sm.prefix; need = sm.need;       // (no barrier after: the next pass writes them two group_syncs later)
     }
     return prefix;
 }
@@ -84,7 +106,7 @@ __device__ __forceinline__ void cta_topk_from_keys(KeyAt key_at, int64_t n, int 
                                                    float* __restrict__ out_val, TopkSmem& sm) {
     const int tid = threadIdx.x;
     unsigned need = (unsigned)k;
-    const unsigned kth = cta_radix_select<4, THREADS>(key_at, n, need, sm.radix);
+    const unsigned kth = radix_select<4, THREADS>(key_at, n, need, sm.radix);
     // ---- gather: strictly greater (any order), then ties in index order
     if (tid == 0) { sm.count = 0; sm.base = 0; }
     __syncthreads();

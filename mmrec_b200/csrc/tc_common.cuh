@@ -117,6 +117,59 @@ __device__ __forceinline__ float fp16_scale_for(uint32_t m_bits) {
     return __uint_as_float((268u - e) << 23);                        // 2^(14 - (e - 127))
 }
 
+// ---- parts of the certified filters (K3 score_cf.cu, K7 knn_cf.cu) -------------------------------------------------
+// One warp per table row of X [n, F]: the largest |element| of the table as an fp32 bit pattern (inf / NaN patterns sort
+// above every finite one, so a non-finite element shows here), atomicMax'ed into *amax; with `rnorm`, also each row's
+// norm, rounded up, into rnorm[r] and the largest of them into *nmax.  Defined in knn_cf.cu.
+__global__ void absmax_norm_kernel(int64_t n, const float* __restrict__ X, int64_t ldx, int F, float* __restrict__ rnorm,
+                                   uint32_t* __restrict__ amax, uint32_t* __restrict__ nmax);
+
+// Operand packing: 8 consecutive elements (k block kb) of row rr of a 128-row tile, times the power of two sc, rounded to
+// fp16 (RN) and stored as 16 bytes at their place in the canonical K-major no-swizzle wgmma layout [tile][kblks][16][8][8],
+// kblks = KP / 8.
+__device__ __forceinline__ void store_fp16x8(uint4* __restrict__ out, int64_t tile, int kblks, int kb, int rr, const float (&x)[8], float sc) {
+    uint32_t w[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const __half2 h = __floats2half2_rn(x[2 * e] * sc, x[2 * e + 1] * sc);
+        w[e] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    out[((tile * kblks + kb) * 16 + rr / 8) * 8 + (rr % 8)] = make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// Pass epilogue: the maxima of the GPT groups of 128 / GPT consecutive columns in one row of an m64n128 accumulator
+// fragment (layout: wgmma.cuh): row half e2 of the quad, whose lane q holds columns 8 j + 2 q + e (j < 16, e < 2).
+// Columns >= n_valid (last item tile) read as -inf.  The quad's lanes shuffle, then, if row < n_rows, lane q stores the
+// groups g with g mod 4 = q to dst()[g], the row's gmax entries.  (Row test and address come after the maxima: formed
+// ahead, they stay live across them and the pass kernels spill more.)
+template <int GPT, class Dst>
+__device__ __forceinline__ void group_max_store(const float (&acc)[64], int e2, int q, int n_valid, int64_t row, int64_t n_rows, Dst dst) {
+    auto val = [&](int j, int e) { return 8 * j + 2 * q + e < n_valid ? acc[4 * j + 2 * e2 + e] : -INFINITY; };
+    float gm[GPT];
+#pragma unroll
+    for (int g = 0; g < GPT; ++g) {
+        float m = -INFINITY;
+#pragma unroll
+        for (int j = g * (16 / GPT); j < (g + 1) * (16 / GPT); ++j) m = fmaxf(m, fmaxf(val(j, 0), val(j, 1)));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        gm[g] = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+    }
+    if (row < n_rows) {
+        float* d = dst();
+#pragma unroll
+        for (int g = 0; g < GPT; ++g)
+            if ((g & 3) == q) d[g] = gm[g];
+    }
+}
+
+// Threshold tail: thr = t - margin and flag 0, or, when t (a NaN / inf group maximum) or the margin (an inf / NaN norm)
+// is not finite, thr = +inf and flag 2: the row takes the exact route.
+__device__ __forceinline__ void set_threshold(float t, float margin, float* thr, int32_t* flag) {
+    const bool finite = fabsf(t) < INFINITY && margin < INFINITY;
+    *thr = finite ? t - margin : INFINITY;
+    *flag = finite ? 0 : 2;
+}
+
 // ---- tile geometry shared by the tensor-core kernels ---------------------------------------------------------
 constexpr int TC_M = 128;          // users per CTA tile: two consumer warpgroups of 64 rows
 constexpr int TC_N = 256;          // items per accumulator (128 fp32 registers per thread)
