@@ -268,6 +268,46 @@ size_t mmrec_knn_topk_workspace_bytes(int64_t n, int F, int64_t m, int k);
 int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k,
                        int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, void* stream);
 int64_t mmrec_debug_knn_fallback_rows(void);
+/* mmrec_knn_topk_shrink_f32: the same, ranked by the shrunk similarity of ItemKNNCBF's `build_item_sim_matrix`
+ *                     (src/models/itemknncbf.py:56-65): v(q, i) = s(q, i) / ((norms[q] * norms[i]) + shrink), s the exact
+ *                     chain above, the denominator two IEEE fp32 roundings (multiply, then add) and an IEEE division.
+ *                     `norms` [n] is the caller's (the reference's `torch.norm(X, p=2, dim=-1)`).  Bit-identical to
+ *                     mmrec_score_f32 on its CUDA-core path, then that elementwise denominator, then mmrec_topk_rows_f32,
+ *                     NaN included.  Uses the workspace of mmrec_knn_topk_workspace_bytes.  Besides the rows the certificate
+ *                     cannot serve, every row takes the exact route when the table holds a non-finite element, when a norm
+ *                     is not finite, when shrink is negative or not finite, or when shrink is 0 and a norm is 0.
+ *                     mmrec_debug_knn_fallback_rows counts them. */
+int mmrec_knn_topk_shrink_f32(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k,
+                              const float* norms, float shrink, int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes,
+                              void* stream);
+
+/* K9  user scores from the sparse interactions and the sparse item kNN graph.   Replaces `scores_matrix = torch.mm(R,
+ * item_sim)` of ItemKNNCBF (src/models/itemknncbf.py:54) and its row gather in full_sort_predict (:107-111) without the
+ * dense [I, I] graph or the dense [U, I] scores.  R [n_users, n_items] and S [n_items, n_items] are int32 CSR (rowptr, col,
+ * val); R's columns ascend within a row, S's columns are distinct within a row.  score[u, j] = the fmaf(R[u, i], S[i, j],
+ * acc) chain over the entries i of R(u) in order, from acc = +0.0; items no S row reaches are +0.0.
+ *
+ * mmrec_sparse_scores_f32: rows users[b] (users == NULL: row b) of that matrix into out [B, n_items] (row stride ldo),
+ *                     overwritten.  Deterministic, no atomics.  Limits: 1 <= n_items < 2^31.
+ * mmrec_sparse_score_topk_f32: the same rows, then `scores[mask_rows, mask_cols] = -1e10` (mask entries: batch row, item;
+ *                     entries outside [0, B) x [0, n_items) are ignored) and the top-k into out_idx / out_val [B, k], with
+ *                     no dense row written.  Bit-identical to mmrec_sparse_scores_f32 + mmrec_mask_f32 +
+ *                     mmrec_topk_rows_f32 (values descending, equal values by ascending index).  Rows with more than 2048
+ *                     products or masked items, or a non-finite score, run that unfused route inside the call.
+ *                     Synchronises `stream`.  Limits: 1 <= k <= min(1024, n_items).
+ * mmrec_sparse_score_topk_workspace_bytes: 0 for arguments outside those limits.
+ * mmrec_debug_sparse_topk_fallback_rows: rows of the last mmrec_sparse_score_topk_f32 call served by the unfused route,
+ *                     -1 before the first call.
+ * ------------------------------------------------------------------------------------------- */
+int mmrec_sparse_scores_f32(int64_t B, const int64_t* users, int64_t n_items, const int32_t* r_ptr, const int32_t* r_col,
+                            const float* r_val, const int32_t* s_ptr, const int32_t* s_col, const float* s_val, float* out,
+                            int64_t ldo, void* stream);
+size_t mmrec_sparse_score_topk_workspace_bytes(int64_t B, int64_t n_items, int64_t mask_nnz, int k);
+int mmrec_sparse_score_topk_f32(int64_t B, const int64_t* users, int64_t n_items, const int32_t* r_ptr, const int32_t* r_col,
+                                const float* r_val, const int32_t* s_ptr, const int32_t* s_col, const float* s_val,
+                                int64_t mask_nnz, const int64_t* mask_rows, const int64_t* mask_cols, int k,
+                                int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, void* stream);
+int64_t mmrec_debug_sparse_topk_fallback_rows(void);
 
 /* K8  full-table exp-sum of LGMRec's hypergraph contrastive loss.   Replaces `ttl_score = torch.exp(torch.matmul(norm_emb1,
  * norm_all_emb.T) / self.tau).sum(dim=1)` of `ssl_triple_loss` (src/models/lgmrec.py:159-166) and its autograd, without the

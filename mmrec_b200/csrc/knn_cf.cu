@@ -51,6 +51,24 @@
 // largest exact value s_k is >= t - eps'.  Every member of the true top-k and every item tied with s_k has s >= s_k, so its
 // s~ >= t - 2 eps' >= thr and its group survives.  The exact ranking of the survivors therefore equals the ranking of all
 // items, ties included.
+//
+// SHRINK ROUTE (mmrec_knn_topk_shrink_f32, ItemKNNCBF: src/models/itemknncbf.py:56-65).  The ranking value is
+// v = s / D, D = fl(fl(nq ni) + shrink) with the caller's norms nq = norms[q], ni = norms[i], and an IEEE division; every
+// returned value is that division of the exact chain (shrink_div).  The three kernels take it as the template parameter
+// SHRINK (the cosine instances are unchanged); the pass epilogue turns each scaled score into v~ = fl((s~ / sc^2) / D)
+// (knn_shrink_tile), the exact route divides its score block elementwise (knn_shrink_rows_kernel).
+// BOUND.  Write A = rnorm[q], B_i = rnorm[i] (the kernel's norms, rounded up), unscaled, E_i = eps(F) A B_i + sub_i the
+// bound above on |s~ / sc^2 - s| (sub_i = sub(F) / sc^2 + the underflow of the two exact power-of-two products).  Then
+//   |v~ - v| <= E_i / D + 2^-24 (|v~| + |v|)                                        (the two divisions round once each),
+//   A B_i / D <= (A / nq)(B_i / ni) (nq ni) / D <= Rq Rmax f (1 + 2^-22),
+// Rq = A / nq, Rmax = max_i B_i / ni (0 for a zero row), and f = nq nmax / (nq nmax + shrink) <= 1: x / (x + shrink) grows with
+// x, so the largest given norm nmax bounds it -- the key fact |q||i| / (|q||i| + shrink) <= 1, which scales eps down by up to
+// shrink / (|q||i| + shrink).  With RR = Rq Rmax f (rounded up), Dmin <= nq nmin + shrink (rounded down, nmin the smallest
+// given norm) and vmax = RR (1 + 2 eps) + sub / Dmin >= |v|, |v~|:
+//   |v~ - v| <= e = eps RR + sub / Dmin + 2^-23 vmax,   thr = t - 2 e (1 + 2^-8),
+// and the certificate above holds with v in place of s.  A negative or non-finite shrink, a non-finite norm, or shrink = 0
+// beside a zero norm (0 / 0) sends every row to the exact route; a NaN / inf margin (a zero norm beside a non-zero row)
+// sends that row.
 #include <cstdio>
 #include <cstdlib>
 
@@ -144,7 +162,42 @@ struct KnnParams {
     int n_pairs, nb, n;                         // query tile pairs and rows of the block, items
     int64_t n_units;
     float* gmax; int G;                         // [nb][G], G = 8 n_it
+    // shrink route only: v = s / (norms[q] norms[i] + shrink); query q = rows ? rows[row] : row_off + row
+    const float* norms; float shrink;
+    const int64_t* rows; int64_t row_off;
+    const uint32_t* header;
 };
+
+// The shrink denominator, two IEEE roundings (multiply, then add) and an IEEE division: `ij.div(i_norm * i_norm.T + shrink)`.
+__device__ __forceinline__ float shrink_div(float s, float nq, float ni, float shrink) {
+    return __fdiv_rn(s, __fadd_rn(__fmul_rn(nq, ni), shrink));
+}
+
+// Shrink route, pass epilogue: this thread's 4 rows x 32 columns of scaled scores s~ become v~ = (s~ / sc^2) / D, D the
+// exact route's denominator.  (1 / sc is a power of two: the two products are exact barring underflow.)
+__device__ __forceinline__ void knn_shrink_tile(const KnnParams& p, float (&acc0)[64], float (&acc1)[64], int row0, int q, int cur_it,
+                                                int n_valid) {
+    const float isc = 1.0f / fp16_scale_for(__ldg(p.header));
+    float qn[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int row = row0 + 64 * (r >> 1) + 8 * (r & 1);
+        qn[r] = row < p.nb ? __ldg(p.norms + (p.rows ? __ldg(p.rows + row) : p.row_off + row)) : 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int c = 8 * j + 2 * q + e;
+            const float ni = c < n_valid ? __ldg(p.norms + (int64_t)cur_it * KN_TILE + c) : 0.f;
+#pragma unroll
+            for (int e2 = 0; e2 < 2; ++e2) {
+                acc0[4 * j + 2 * e2 + e] = shrink_div(acc0[4 * j + 2 * e2 + e] * isc * isc, qn[e2], ni, p.shrink);
+                acc1[4 * j + 2 * e2 + e] = shrink_div(acc1[4 * j + 2 * e2 + e] * isc * isc, qn[2 + e2], ni, p.shrink);
+            }
+        }
+    }
+}
 
 __device__ __forceinline__ void knn_producer(const KnnParams& p, uint32_t sbase, int64_t u0, int64_t u1) {
     const uint32_t bar = sbase + KN_BARS;
@@ -168,6 +221,7 @@ __device__ __forceinline__ void knn_producer(const KnnParams& p, uint32_t sbase,
     }
 }
 
+template <bool SHRINK>
 __device__ __forceinline__ void knn_consumer(const KnnParams& p, uint32_t sbase, int64_t u0, int64_t u1, int h) {
     const uint32_t bar = sbase + KN_BARS;
     constexpr uint32_t LBO = (KN_TILE / 8) * 128, SBO = 128;
@@ -215,6 +269,7 @@ __device__ __forceinline__ void knn_consumer(const KnnParams& p, uint32_t sbase,
         // ---- epilogue: maxima of the 8 groups of 16 columns of rows row0 + 8 e2 (acc0) and row0 + 64 + 8 e2 (acc1)
         const int n_valid = p.n - cur_it * KN_TILE;
         const int row0 = base + 16 * w + (lane >> 2);
+        if constexpr (SHRINK) knn_shrink_tile(p, acc0, acc1, row0, q, cur_it, n_valid);
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
             const int row = row0 + 64 * (r >> 1) + 8 * (r & 1);
@@ -224,6 +279,7 @@ __device__ __forceinline__ void knn_consumer(const KnnParams& p, uint32_t sbase,
     }
 }
 
+template <bool SHRINK>
 __global__ void __launch_bounds__(KN_THREADS, 1) knn_pass_kernel(const KnnParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     const uint32_t sbase = smem_u32(smem);
@@ -245,16 +301,18 @@ __global__ void __launch_bounds__(KN_THREADS, 1) knn_pass_kernel(const KnnParams
         if (warp == KN_CONSUMER_WARPS && lane == 0) knn_producer(p, sbase, u0, u1);
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-        knn_consumer(p, sbase, u0, u1, warp >> 2);
+        knn_consumer<SHRINK>(p, sbase, u0, u1, warp >> 2);
     }
 }
 
 // ---- threshold ------------------------------------------------------------------------------------------------------
 // One CTA per row.  Radix select (radix_select, select.cuh) over the keys of the row's group maxima, top 24 bits: the
 // result is the lower edge of the bucket holding the k-th largest maximum, so at least k maxima are >= it.
+template <bool SHRINK>
 __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int64_t G_valid, int k, int F, const float* __restrict__ gmax,
                                                       const int64_t* __restrict__ rows, int64_t row_off, const float* __restrict__ rnorm,
-                                                      const uint32_t* __restrict__ header, float* __restrict__ thr, int32_t* __restrict__ flags) {
+                                                      const uint32_t* __restrict__ header, float* __restrict__ thr, int32_t* __restrict__ flags,
+                                                      const float* __restrict__ norms, float shrink) {
     __shared__ RadixSmem sm;
     const int64_t row = blockIdx.x;
     const int tid = threadIdx.x;
@@ -266,7 +324,25 @@ __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int
     const float* g = gmax + row * G;
     unsigned need = (unsigned)k;
     const unsigned prefix = radix_select<3, 256>([=](int64_t i) { return float_key(__ldg(g + i)); }, G_valid, need, sm);
-    if (tid == 0) {
+    if (SHRINK && tid == 0) {
+        // header words: [0] largest |element|, [1] largest rnorm, [2] largest rnorm[i] / norms[i] (rounded up), [3] 0x7fffffff
+        // minus the bits of the smallest norms[i], [5] the largest norms[i]
+        const float isc = 1.0f / fp16_scale_for(header[0]);
+        const int64_t qrow = rows ? rows[row] : row_off + row;
+        const float A = rnorm[qrow], nq = norms[qrow], Bm = __uint_as_float(header[1]);
+        const float Rmax = __uint_as_float(header[2]), nmin = __uint_as_float(0x7fffffffu - header[3]);
+        const float nmx = __uint_as_float(header[5]);
+        // |q||i| / D_i <= Rq R_i (nq ni) / D_i, and nq ni / (nq ni + shrink) grows with ni: at most its value at the largest norm
+        const float fac = __fdiv_ru(__fmul_ru(nq, nmx), __fadd_rd(__fmul_rd(nq, nmx), shrink));
+        const float RR = __fmul_ru(__fmul_ru(A == 0.f ? 0.f : __fdiv_ru(A, nq), Rmax), fac) * (1.0f + 0x1p-20f);
+        const float Dmin = __fmul_rd(__fadd_rd(__fmul_rd(nq, nmin), shrink), 1.0f - 0x1p-22f);
+        const float steps = (float)((F + KN_KC - 1) / KN_KC * (KN_KC / 16));
+        const float eps = 0x1p-10f + 0x1p-22f + (steps * 0x1p-22f + (float)F * 0x1p-24f) * (1.0f + 0x1p-9f);
+        const float sub = (0x1p-25f * sqrtf((float)F) * (A + Bm) * isc + (float)F * 0x1p-50f * isc * isc + 0x1p-120f) / Dmin;
+        const float vmax = RR * (1.0f + 2.0f * eps) + sub;
+        set_threshold(key_float(prefix), 2.0f * (eps * RR + sub + 0x1p-23f * vmax) * (1.0f + 0x1p-8f), thr + row, flags + row);
+    }
+    if (!SHRINK && tid == 0) {
         const float sc = fp16_scale_for(header[0]);
         const int64_t qrow = rows ? rows[row] : row_off + row;
         const float un = rnorm[qrow] * sc, mn = __uint_as_float(header[1]) * sc;
@@ -302,12 +378,14 @@ __device__ __forceinline__ float knn_exact(const float* __restrict__ q, const fl
     return acc;
 }
 
+template <bool SHRINK>
 __global__ void __launch_bounds__(KN_FIN_THREADS) knn_final_kernel(int64_t nb, int64_t n, const float* __restrict__ X, int64_t ldx, int F, int k,
                                                                    const int64_t* __restrict__ rows, int64_t row_off, int64_t G_valid,
                                                                    const float* __restrict__ gmax, int64_t G, const float* __restrict__ thr,
                                                                    const int32_t* __restrict__ flags, int32_t* __restrict__ counter,
                                                                    int64_t* __restrict__ fb_rows, int64_t* __restrict__ fb_pos,
-                                                                   int64_t* __restrict__ out_idx, float* __restrict__ out_val) {
+                                                                   int64_t* __restrict__ out_idx, float* __restrict__ out_val,
+                                                                   const float* __restrict__ norms, float shrink) {
     __shared__ uint64_t comp[KN_CAP];
     __shared__ int32_t glist[KN_CAP / KN_GROUP];
     __shared__ int s_cnt;
@@ -344,7 +422,11 @@ __global__ void __launch_bounds__(KN_FIN_THREADS) knn_final_kernel(int64_t nb, i
         uint64_t v = 0;                                                // (padding: below every real composite)
         if (c < nc) {
             const int64_t item = (int64_t)glist[c / KN_GROUP] * KN_GROUP + (c % KN_GROUP);
-            if (item < n) v = ((uint64_t)float_key(knn_exact(qv, X + item * ldx, F, vec)) << 32) | (uint32_t)(~(uint32_t)item);
+            if (item < n) {
+                float s = knn_exact(qv, X + item * ldx, F, vec);
+                if constexpr (SHRINK) s = shrink_div(s, __ldg(norms + qrow), __ldg(norms + item), shrink);
+                v = ((uint64_t)float_key(s) << 32) | (uint32_t)(~(uint32_t)item);
+            }
         }
         comp[c] = v;
     }
@@ -363,6 +445,41 @@ __global__ void knn_scatter_kernel(int64_t cnt, int k, const int64_t* __restrict
     const int64_t s = t / k, j = t - s * k;
     out_idx[pos[s] * k + j] = idx_in[t];
     out_val[pos[s] * k + j] = val_in[t];
+}
+
+// Shrink route: the exact route's elementwise denominator on a score block (row j = table row src[j], or row0 + j).
+__global__ void knn_shrink_rows_kernel(int64_t c, int64_t n, float* __restrict__ S, const int64_t* __restrict__ src, int64_t row0,
+                                       const float* __restrict__ norms, float shrink) {
+    const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (t >= c * n) return;
+    const int64_t j = t / n, i = t - j * n;
+    S[t] = shrink_div(S[t], __ldg(norms + (src ? __ldg(src + j) : row0 + j)), __ldg(norms + i), shrink);
+}
+
+// Shrink route, table summary of the given norms next to the kernel's own (rounded-up) ones: header[2] = the largest
+// rnorm[i] / norms[i] rounded up (0 for a zero row; inf / NaN when a norm is 0 or NaN beside a non-zero row), header[3] =
+// 0x7fffffff minus the bits of the smallest norms[i], header[4] = 1 if any norms[i] is not finite, header[5] = the largest
+// norms[i].
+__global__ void knn_shrink_prep_kernel(int64_t n, const float* __restrict__ rnorm, const float* __restrict__ norms, uint32_t* __restrict__ header) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    uint32_t ratio = 0u, nmin = 0u, bad = 0u, nmax = 0u;
+    if (i < n) {
+        const float r = rnorm[i], ni = norms[i];
+        ratio = __float_as_uint(r == 0.f ? 0.f : __fdiv_ru(r, ni)) & 0x7fffffffu;
+        nmin = 0x7fffffffu - (__float_as_uint(ni) & 0x7fffffffu);
+        bad = !(fabsf(ni) < INFINITY);
+        nmax = bad ? 0u : __float_as_uint(ni) & 0x7fffffffu;
+    }
+    ratio = __reduce_max_sync(0xffffffffu, ratio);
+    nmin = __reduce_max_sync(0xffffffffu, nmin);
+    bad = __reduce_or_sync(0xffffffffu, bad);
+    nmax = __reduce_max_sync(0xffffffffu, nmax);
+    if ((threadIdx.x & 31) == 0) {
+        if (ratio) atomicMax(header + 2, ratio);
+        if (nmin) atomicMax(header + 3, nmin);
+        if (bad) atomicOr(header + 4, 1u);
+        if (nmax) atomicMax(header + 5, nmax);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -416,7 +533,8 @@ static int64_t g_knn_fallback_rows = -1;
 // The existing route for `cnt` query rows (table rows src_rows[j], or row0 + j when src_rows is NULL): exact fp32 scores of
 // gemm_nt_kernel into the score block, mmrec_topk_rows_f32, then rows j go to output rows dst_pos[j] (or row0 + j).
 static int knn_exact_rows(int64_t cnt, const int64_t* src_rows, const int64_t* dst_pos, int64_t row0, int64_t n, const float* X, int64_t ldx,
-                          int F, int k, const KnnPlan& P, char* base, int64_t* out_idx, float* out_val, cudaStream_t stream) {
+                          int F, int k, const KnnPlan& P, char* base, int64_t* out_idx, float* out_val, cudaStream_t stream,
+                          const float* norms = nullptr, float shrink = 0.f) {
     float* S = (float*)(base + P.off_s);
     int64_t* ti = (int64_t*)(base + P.off_ti);
     float* tv = (float*)(base + P.off_tv);
@@ -427,6 +545,11 @@ static int knn_exact_rows(int64_t cnt, const int64_t* src_rows, const int64_t* d
         g.B = X; g.ldb = ldx; g.N = n; g.K = F; g.bias = nullptr; g.C = S; g.ldc = n; g.l2_normalize = 0;
         int rc = launch_gemm_nt<128, 128, 8, 8>(g, stream);
         if (rc) return rc;
+        if (norms) {
+            knn_shrink_rows_kernel<<<(unsigned)((c * n + 255) / 256), 256, 0, stream>>>(c, n, S, src_rows ? src_rows + c0 : nullptr, row0 + c0,
+                                                                                      norms, shrink);
+            MMREC_LAUNCH_CHECK();
+        }
         if (dst_pos) {
             rc = mmrec_topk_rows_f32(c, n, S, n, k, 0, ti, tv, stream);
             if (rc) return rc;
@@ -451,9 +574,25 @@ extern "C" size_t mmrec_knn_topk_workspace_bytes(int64_t n, int F, int64_t m, in
 
 extern "C" int64_t mmrec_debug_knn_fallback_rows(void) { return g_knn_fallback_rows; }
 
+template <bool SHRINK>
+static int knn_topk_impl(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k, const float* norms,
+                         float shrink, int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, cudaStream_t stream);
+
 extern "C" int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k,
                                   int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, void* stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
+    return knn_topk_impl<false>(n, X, ldx, F, m, rows, k, nullptr, 0.f, out_idx, out_val, ws, ws_bytes, (cudaStream_t)stream_);
+}
+
+extern "C" int mmrec_knn_topk_shrink_f32(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k,
+                                         const float* norms, float shrink, int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes,
+                                         void* stream_) {
+    MMREC_CHECK_ARG(norms != nullptr || m == 0, "knn_topk_shrink: null norms");
+    return knn_topk_impl<true>(n, X, ldx, F, m, rows, k, norms, shrink, out_idx, out_val, ws, ws_bytes, (cudaStream_t)stream_);
+}
+
+template <bool SHRINK>
+static int knn_topk_impl(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k, const float* norms,
+                         float shrink, int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, cudaStream_t stream) {
     MMREC_CHECK_ARG(n >= 1 && F >= 1 && m >= 0, "knn_topk: bad sizes (need n >= 1, F >= 1, m >= 0)");
     MMREC_CHECK_ARG(k >= 1 && k <= 1024 && k <= n, "knn_topk: need 1 <= k <= min(1024, n)");
     MMREC_CHECK_ARG(n < (1ll << 31), "knn_topk: n must fit 31 bits");
@@ -470,7 +609,7 @@ extern "C" int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F,
     int dev = 0;
     MMREC_CUDA(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !attr_done[dev]) {
-        MMREC_CUDA(cudaFuncSetAttribute(knn_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KN_SMEM));
+        MMREC_CUDA(cudaFuncSetAttribute(knn_pass_kernel<SHRINK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KN_SMEM));
         if (dev >= 0 && dev < 64) attr_done[dev] = true;
     }
     uint32_t* header = (uint32_t*)(base + P.off_hdr);
@@ -491,11 +630,17 @@ extern "C" int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F,
         absmax_norm_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, stream>>>(n, X, ldx, F, rnorm, header, header + 1);
         MMREC_LAUNCH_CHECK();
     }
-    uint32_t h_amax = 0;
-    MMREC_CUDA(cudaMemcpyAsync(&h_amax, header, 4, cudaMemcpyDeviceToHost, stream));
+    if (SHRINK) {
+        knn_shrink_prep_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(n, rnorm, norms, header);
+        MMREC_LAUNCH_CHECK();
+    }
+    uint32_t h[5] = {0, 0, 0, 0, 0};
+    MMREC_CUDA(cudaMemcpyAsync(h, header, sizeof(h), cudaMemcpyDeviceToHost, stream));
     MMREC_CUDA(cudaStreamSynchronize(stream));
-    if (h_amax >= 0x7f800000u) {
-        int rc = knn_exact_rows(m, rows, nullptr, 0, n, X, ldx, F, k, P, base, out_idx, out_val, stream);
+    // shrink route: the certificate needs a finite shrink >= 0, finite norms and, with shrink 0, no zero norm (0 / 0)
+    const bool shrink_exact = SHRINK && (!(shrink >= 0.f && shrink < INFINITY) || h[4] || (shrink == 0.f && h[3] == 0x7fffffffu));
+    if (h[0] >= 0x7f800000u || shrink_exact) {
+        int rc = knn_exact_rows(m, rows, nullptr, 0, n, X, ldx, F, k, P, base, out_idx, out_val, stream, norms, shrink);
         if (rc) return rc;
         g_knn_fallback_rows = m;
         return MMREC_OK;
@@ -522,19 +667,22 @@ extern "C" int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F,
         p.Qpk = Qpk; p.Xpk = Xpk; p.KP = P.KP; p.nc = P.KP / KN_KC;
         p.n_pairs = (int)(nb_pad / (2 * KN_TILE)); p.n_units = p.n_pairs * P.n_it; p.nb = (int)nb; p.n = (int)n;
         p.gmax = gmax; p.G = (int)P.G;
+        p.norms = norms; p.shrink = shrink; p.rows = rb; p.row_off = r0; p.header = header;
         const unsigned grid = (unsigned)(p.n_units < sms ? p.n_units : sms);
-        knn_pass_kernel<<<grid, KN_THREADS, KN_SMEM, stream>>>(p);
+        knn_pass_kernel<SHRINK><<<grid, KN_THREADS, KN_SMEM, stream>>>(p);
         MMREC_LAUNCH_CHECK();
-        knn_thr_kernel<<<(unsigned)nb, 256, 0, stream>>>(nb, P.G, P.G_valid, k, F, gmax, rb, r0, rnorm, header, thr, flags);
+        knn_thr_kernel<SHRINK><<<(unsigned)nb, 256, 0, stream>>>(nb, P.G, P.G_valid, k, F, gmax, rb, r0, rnorm, header, thr, flags, norms, shrink);
         MMREC_LAUNCH_CHECK();
-        knn_final_kernel<<<(unsigned)nb, KN_FIN_THREADS, 0, stream>>>(nb, n, X, ldx, F, k, rb, r0, P.G_valid, gmax, P.G, thr, flags, counter,
-                                                                      fb_rows, fb_pos, out_idx + r0 * k, out_val + r0 * k);
+        knn_final_kernel<SHRINK><<<(unsigned)nb, KN_FIN_THREADS, 0, stream>>>(nb, n, X, ldx, F, k, rb, r0, P.G_valid, gmax, P.G, thr, flags,
+                                                                              counter, fb_rows, fb_pos, out_idx + r0 * k, out_val + r0 * k,
+                                                                              norms, shrink);
         MMREC_LAUNCH_CHECK();
         int32_t cnt = 0;
         MMREC_CUDA(cudaMemcpyAsync(&cnt, counter, 4, cudaMemcpyDeviceToHost, stream));
         MMREC_CUDA(cudaStreamSynchronize(stream));
         if (cnt > 0) {
-            int rc = knn_exact_rows(cnt, fb_rows, fb_pos, 0, n, X, ldx, F, k, P, base, out_idx + r0 * k, out_val + r0 * k, stream);
+            int rc = knn_exact_rows(cnt, fb_rows, fb_pos, 0, n, X, ldx, F, k, P, base, out_idx + r0 * k, out_val + r0 * k, stream, norms,
+                                    shrink);
             if (rc) return rc;
             n_fb += cnt;
         }

@@ -735,12 +735,17 @@ def fused_stage_times():
     return [float(buf[i]) for i in range(n)]
 
 
-def knn_topk(x: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None):
+def knn_topk(x: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None, norms: Optional[torch.Tensor] = None,
+             shrink: Optional[float] = None):
     """Top-k of `x[rows] @ x.T` per query row (all rows by default) without the [m, n] similarity matrix
     (`mmrec_knn_topk_f32`, K7): the cosine kNN of `src/models/freedom.py:79-91` / `src/utils/utils.py:165-172` for the
     normalised feature table `x`.  Returns (values [m, k], indices int64 [m, k]), bit-identical to `score(x[rows], x)`
-    followed by `mask_topk(.., None, k)` on the CUDA-core path."""
-    _need_cuda(x, rows)
+    followed by `mask_topk(.., None, k)` on the CUDA-core path.
+
+    With `shrink` (`mmrec_knn_topk_shrink_f32`): ranked by `(x[q] . x[i]) / (norms[q] * norms[i] + shrink)`, ItemKNNCBF's
+    `build_item_sim_matrix` (`src/models/itemknncbf.py:56-65`); `norms` defaults to `torch.norm(x, p=2, dim=-1)`, the
+    reference's expression.  Bit-identical to the score, that elementwise denominator, then `mask_topk(.., None, k)`."""
+    _need_cuda(x, rows, norms)
     lib = _lib.load()
     if x.dim() != 2:
         raise MMRecError("knn_topk: x must be [n, F]")
@@ -760,8 +765,15 @@ def knn_topk(x: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None):
     if m == 0:
         return val, idx
     ws = _ws("knn", lib.mmrec_knn_topk_workspace_bytes(n, F, m, k) + 1024, x.device)
-    check(lib.mmrec_knn_topk_f32(n, _ptr(x), x.stride(0), F, m, _ptr(rows), k, _ptr(idx), _ptr(val), _ptr(ws), ws.numel(), _stream()),
-          "mmrec_knn_topk_f32")
+    if shrink is None:
+        check(lib.mmrec_knn_topk_f32(n, _ptr(x), x.stride(0), F, m, _ptr(rows), k, _ptr(idx), _ptr(val), _ptr(ws), ws.numel(),
+                                     _stream()), "mmrec_knn_topk_f32")
+    else:
+        norms = torch.norm(x, p=2, dim=-1) if norms is None else _f32c(norms)
+        if norms.shape != (n,):
+            raise MMRecError(f"knn_topk: norms must be [{n}]")
+        check(lib.mmrec_knn_topk_shrink_f32(n, _ptr(x), x.stride(0), F, m, _ptr(rows), k, _ptr(norms), float(shrink), _ptr(idx),
+                                            _ptr(val), _ptr(ws), ws.numel(), _stream()), "mmrec_knn_topk_shrink_f32")
     # the graphs are built once, at model construction: the scratch (2 n F bytes of fp16 pack) is not kept for later calls
     # (the call has synchronised the stream, so the memory is free to go back to the allocator)
     _ws_cache.pop(("knn", x.device.index, torch.cuda.current_stream(x.device).cuda_stream), None)
@@ -772,6 +784,61 @@ def knn_fallback_rows() -> int:
     """Diagnostic: rows of the last `knn_topk` call that took the exact route (all of them when the table held a
     non-finite element); -1 before the first call."""
     return int(_lib.load().mmrec_debug_knn_fallback_rows())
+
+
+# ------------------------------------------------------------------------------------------------
+# K9: user scores from the sparse interactions and the sparse item kNN graph (ItemKNNCBF)
+# ------------------------------------------------------------------------------------------------
+def _sparse_pair(R: CSR, S: CSR, users):
+    if R.n_cols != S.n_rows or S.n_rows != S.n_cols:
+        raise MMRecError(f"sparse scores: R [{R.n_rows}, {R.n_cols}] and S [{S.n_rows}, {S.n_cols}] do not chain")
+    _need_cuda(R.rowptr, S.rowptr, users)
+    if users is not None:
+        users = users.to(torch.int64).contiguous()
+    return users, (R.rowptr, R.colidx, _f32c(R.vals), S.rowptr, S.colidx, _f32c(S.vals))
+
+
+def sparse_scores(R: CSR, S: CSR, users: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Rows `users` of `R @ S` as a fresh dense fp32 [B, n_items] owned by the caller (the trainer mutates it):
+    `self.scores_matrix[user]` with `scores_matrix = torch.mm(r_matrix, item_sim)` (`src/models/itemknncbf.py:54`,
+    `:107-111`), summed per element over R's row in ascending column order (`mmrec_sparse_scores_f32`, K9)."""
+    users, parts = _sparse_pair(R, S, users)
+    B = R.n_rows if users is None else users.numel()
+    out = torch.empty(B, S.n_cols, dtype=torch.float32, device=R.rowptr.device)
+    check(_lib.load().mmrec_sparse_scores_f32(B, _ptr(users), S.n_cols, *(_ptr(t) for t in parts), _ptr(out), S.n_cols, _stream()),
+          "mmrec_sparse_scores_f32")
+    return out
+
+
+def sparse_score_topk(R: CSR, S: CSR, users: Optional[torch.Tensor], mask: Optional[torch.Tensor], k: int):
+    """Fused `sparse_scores` + `scores[mask[0], mask[1]] = -1e10` + top-k (`src/common/trainer.py:304-309`) without a
+    dense row (`mmrec_sparse_score_topk_f32`, K9).  Returns (values [B, k], indices int64 [B, k]), bit-identical to
+    `mask_topk(sparse_scores(R, S, users), mask, k)`."""
+    users, parts = _sparse_pair(R, S, users)
+    _need_cuda(mask)
+    lib = _lib.load()
+    B = R.n_rows if users is None else users.numel()
+    n_items = S.n_cols
+    if not (1 <= k <= min(1024, n_items)):
+        raise MMRecError(f"sparse_score_topk: need 1 <= k <= min(1024, n_items = {n_items}), got {k}")
+    m0 = m1 = None
+    nnz = 0
+    if mask is not None and mask.numel() > 0:
+        mask = mask.to(torch.int64).contiguous()
+        m0, m1, nnz = mask[0], mask[1], mask.shape[1]
+    dev = R.rowptr.device
+    idx = torch.empty(B, k, dtype=torch.int64, device=dev)
+    val = torch.empty(B, k, dtype=torch.float32, device=dev)
+    ws = _ws("sparse_topk", lib.mmrec_sparse_score_topk_workspace_bytes(B, n_items, nnz, k), dev)
+    check(lib.mmrec_sparse_score_topk_f32(B, _ptr(users), n_items, *(_ptr(t) for t in parts), nnz, _ptr(m0), _ptr(m1), k, _ptr(idx),
+                                          _ptr(val), _ptr(ws), ws.numel(), _stream()), "mmrec_sparse_score_topk_f32")
+    return val, idx
+
+
+def sparse_topk_fallback_rows() -> int:
+    """Diagnostic: rows of the last `sparse_score_topk` call served by the unfused route (too many products or masked
+    items for shared memory, or a non-finite score); -1 before the first call."""
+    return int(_lib.load().mmrec_debug_sparse_topk_fallback_rows())
 
 
 # ------------------------------------------------------------------------------------------------
