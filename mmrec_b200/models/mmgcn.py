@@ -23,9 +23,15 @@ from ..common.abstract_recommender import GeneralRecommender
 from ..ops import CSR
 
 
-def mean_adj_from_edges(edge_index: torch.Tensor, n_nodes: int) -> CSR:
-    """Row-normalised adjacency of PyG's mean aggregation: out[dst] = mean over edges (src -> dst) of x[src]."""
+def mean_adj_from_edges(edge_index: torch.Tensor, n_nodes: int, self_loops: bool = False) -> CSR:
+    """Row-normalised adjacency of PyG's mean aggregation: out[dst] = mean over edges (src -> dst) of x[src].
+    `self_loops`: PyG's `remove_self_loops` then `add_self_loops` first, so every node counts itself once (MVGAE's
+    `BaseModel.forward`, `src/models/mvgae.py:323-326`)."""
     src, dst = edge_index[0], edge_index[1]
+    if self_loops:
+        keep = src != dst
+        loop = torch.arange(n_nodes, dtype=src.dtype, device=src.device)
+        src, dst = torch.cat((src[keep], loop)), torch.cat((dst[keep], loop))
     deg = torch.zeros(n_nodes, dtype=torch.float32, device=src.device).index_add_(0, dst, torch.ones_like(dst, dtype=torch.float32))
     vals = 1.0 / deg[dst]
     return CSR.from_coo(dst, src, vals, n_nodes, n_nodes, sum_duplicates=True, symmetric=False)

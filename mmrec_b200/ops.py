@@ -715,6 +715,44 @@ def score_topk(user_e, item_e, users, mask, k: int, item_offset: int = 0, out=No
     return val, idx
 
 
+class _MaxDotFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, t):
+        val, idx = score_topk(q, t, None, None, 1)
+        val, idx = val.view(-1), idx.view(-1)
+        ctx.save_for_backward(q, t, idx)
+        ctx.mark_non_differentiable(idx)
+        return val, idx
+
+    @staticmethod
+    def backward(ctx, g, _g_idx):
+        # the gradient of a max reaches the selected pair only: O(B d), no [B, M] or [B, M, d] tensor
+        q, t, idx = ctx.saved_tensors
+        g = _f32c(g).unsqueeze(1)
+        dq = g * t[idx] if ctx.needs_input_grad[0] else None
+        dt = index_sum_rows(g * q, idx, t.shape[0]) if ctx.needs_input_grad[1] else None
+        return dq, dt
+
+
+def max_dot(q: torch.Tensor, t: torch.Tensor):
+    """`torch.max(torch.sum(q[:, None, :] * t[None, :, :], -1), dim=-1)` without the [B, M, d] product or the [B, M] scores:
+    MVGAE's hardest in-batch negative (`src/models/mvgae.py:73-85`, which builds `z[users.repeat(1, B)] * z[neg_items]`).
+    q [B, d] and t [M, d] are fp32 device tensors.  Returns (values [B], index int64 [B]): values[b] is the largest
+    `<q_b, t_j>` in the fp32 chain of `score_topk` (K3, k = 1), index[b] the lowest j that reaches it.  Only `values` is
+    differentiable: dq = g t[index], dt = index_sum_rows(g q, index, M) (contributions to a row of t summed in ascending b,
+    so the gradient is bit-reproducible).  Memory: O(B d) per call; the scratch is `score_topk`'s cached workspace, shared
+    with the evaluation and bounded (its unfused route's score block is capped at 64 MiB).
+
+    NaN: the chain's NaN is the positive canonical NaN, which K3's key order ranks above +inf, and equal keys go to the
+    lowest index; so a row with a NaN score returns NaN at its first NaN column, as `torch.max` does (whatever the sign
+    bit of the NaN that went into q or t).  Scores are never -0.0 (the chain starts from +0.0), so +0.0 and -0.0 never
+    compete."""
+    _need_cuda(q, t)
+    if q.dim() != 2 or t.dim() != 2 or q.shape[1] != t.shape[1] or t.shape[0] < 1:
+        raise MMRecError(f"max_dot: q {tuple(q.shape)} and t {tuple(t.shape)} must be [B, d] and [M >= 1, d]")
+    return _MaxDotFn.apply(q, t)
+
+
 _last_fused: dict = {}
 
 
