@@ -38,6 +38,20 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 // number of SMs of the current device (cached)
 int sm_count();
 
+// Opts the kernels in to `bytes` of dynamic shared memory, once per device (the attribute is per device).
+template <auto... Kernels>
+int set_smem_once(int bytes) {
+    static bool done[64] = {false};
+    int dev = 0;
+    MMREC_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= 64 || !done[dev]) {
+        for (const void* kernel : {(const void*)Kernels...})
+            MMREC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        if (dev >= 0 && dev < 64) done[dev] = true;
+    }
+    return MMREC_OK;
+}
+
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
 __device__ __forceinline__ float warp_sum(float v) {

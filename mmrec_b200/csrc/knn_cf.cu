@@ -26,9 +26,9 @@
 //                       from the original fp32 rows) -> bitonic sort on (float_key, ~index) -> top-k.
 //   exact route         rows the filter does not serve (fewer than k groups, more than KN_CAP candidates, a non-finite
 //                       margin) are listed; after each row block the host reads the count and runs the existing route on
-//                       them: gemm_nt_kernel (gemm_simt.cuh, the same template instance as mmrec_score_f32) on the gathered
-//                       rows + mmrec_topk_rows_f32, then a scatter.  Bit-identical by construction.  A table with any
-//                       non-finite element (a zero row normalises to NaN) takes that route for every row.
+//                       them (exact_rows.cuh): gemm_nt_kernel (gemm_simt.cuh, the same template instance as mmrec_score_f32)
+//                       on the gathered rows + mmrec_topk_rows_f32, then a scatter.  Bit-identical by construction.  A
+//                       table with any non-finite element (a zero row normalises to NaN) takes that route for every row.
 //
 // ERROR BOUND (scaled domain: a = sc X[q], b = sc X[i]; the exact value s is the fp32 chain above times sc^2, exact for a
 // power of two barring underflow).  Write s* for the real dot product a . b.
@@ -72,6 +72,7 @@
 #include <cstdio>
 #include <cstdlib>
 
+#include "exact_rows.cuh"
 #include "gemm_simt.cuh"
 #include "select.cuh"
 #include "tc_common.cuh"
@@ -438,15 +439,6 @@ __global__ void __launch_bounds__(KN_FIN_THREADS) knn_final_kernel(int64_t nb, i
     }
 }
 
-__global__ void knn_scatter_kernel(int64_t cnt, int k, const int64_t* __restrict__ pos, const int64_t* __restrict__ idx_in,
-                                   const float* __restrict__ val_in, int64_t* __restrict__ out_idx, float* __restrict__ out_val) {
-    const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (t >= cnt * k) return;
-    const int64_t s = t / k, j = t - s * k;
-    out_idx[pos[s] * k + j] = idx_in[t];
-    out_val[pos[s] * k + j] = val_in[t];
-}
-
 // Shrink route: the exact route's elementwise denominator on a score block (row j = table row src[j], or row0 + j).
 __global__ void knn_shrink_rows_kernel(int64_t c, int64_t n, float* __restrict__ S, const int64_t* __restrict__ src, int64_t row0,
                                        const float* __restrict__ norms, float shrink) {
@@ -488,7 +480,7 @@ __global__ void knn_shrink_prep_kernel(int64_t n, const float* __restrict__ rnor
 struct KnnPlan {
     int KP;
     int64_t n_it, G, G_valid, rows_blk, rows_pad, s_rows;
-    size_t off_hdr, off_xpk, off_rnorm, off_qpk, off_gmax, off_thr, off_flags, off_cnt, off_fbr, off_fbp, off_s, off_ti, off_tv, total;
+    size_t off_hdr, off_xpk, off_rnorm, off_qpk, off_gmax, off_thr, off_flags, off_cnt, off_fbr, off_fbp, off_ex, total;
 };
 
 static KnnPlan knn_plan(int64_t n, int F, int64_t m, int k) {
@@ -504,11 +496,7 @@ static KnnPlan knn_plan(int64_t n, int F, int64_t m, int k) {
     const int64_t m_pad = (m + 2 * KN_TILE - 1) / (2 * KN_TILE) * (2 * KN_TILE);
     P.rows_blk = m_pad < rb ? m_pad : rb;
     P.rows_pad = P.rows_blk;                                          // (a multiple of 256)
-    // score block of the exact route: <= 256 MB, at most 1024 rows
-    int64_t sr = (256ll << 20) / (4 * n);
-    if (sr < 1) sr = 1;
-    if (sr > 1024) sr = 1024;
-    P.s_rows = sr;
+    P.s_rows = exact_block_rows(n, m);
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes > 0 ? bytes : 1, 1024); return o; };
     P.off_hdr = take(1024);
@@ -521,46 +509,27 @@ static KnnPlan knn_plan(int64_t n, int F, int64_t m, int k) {
     P.off_cnt = take(4);
     P.off_fbr = take((size_t)P.rows_blk * 8);
     P.off_fbp = take((size_t)P.rows_blk * 8);
-    P.off_s = take((size_t)P.s_rows * n * 4);
-    P.off_ti = take((size_t)P.s_rows * k * 8);
-    P.off_tv = take((size_t)P.s_rows * k * 4);
+    P.off_ex = take(exact_rows_bytes(P.s_rows, n, k));
     P.total = off + 1024;
     return P;
 }
 
 static int64_t g_knn_fallback_rows = -1;
 
-// The existing route for `cnt` query rows (table rows src_rows[j], or row0 + j when src_rows is NULL): exact fp32 scores of
-// gemm_nt_kernel into the score block, mmrec_topk_rows_f32, then rows j go to output rows dst_pos[j] (or row0 + j).
-static int knn_exact_rows(int64_t cnt, const int64_t* src_rows, const int64_t* dst_pos, int64_t row0, int64_t n, const float* X, int64_t ldx,
-                          int F, int k, const KnnPlan& P, char* base, int64_t* out_idx, float* out_val, cudaStream_t stream,
-                          const float* norms = nullptr, float shrink = 0.f) {
-    float* S = (float*)(base + P.off_s);
-    int64_t* ti = (int64_t*)(base + P.off_ti);
-    float* tv = (float*)(base + P.off_tv);
-    for (int64_t c0 = 0; c0 < cnt; c0 += P.s_rows) {
-        const int64_t c = cnt - c0 < P.s_rows ? cnt - c0 : P.s_rows;
+// The existing route for `cnt` query rows (table rows src_rows[j], or j when src_rows is NULL): exact fp32 scores of
+// gemm_nt_kernel (+ the shrink division), mmrec_topk_rows_f32, then rows j go to output rows dst_pos[j] (or j).
+static int knn_exact_rows(int64_t cnt, const int64_t* src_rows, const int64_t* dst_pos, int64_t n, const float* X, int64_t ldx, int F, int k,
+                          const KnnPlan& P, char* base, int64_t* out_idx, float* out_val, cudaStream_t stream, const float* norms, float shrink) {
+    return exact_rows_topk(cnt, dst_pos, n, k, P.s_rows, base + P.off_ex, out_idx, out_val, stream, [&](int64_t c0, int64_t c, float* S) {
         GemmNT g;
-        g.A = src_rows ? X : X + (row0 + c0) * ldx; g.lda = ldx; g.a_idx = src_rows ? src_rows + c0 : nullptr; g.M = c;
+        g.A = src_rows ? X : X + c0 * ldx; g.lda = ldx; g.a_idx = src_rows ? src_rows + c0 : nullptr; g.M = c;
         g.B = X; g.ldb = ldx; g.N = n; g.K = F; g.bias = nullptr; g.C = S; g.ldc = n; g.l2_normalize = 0;
         int rc = launch_gemm_nt<128, 128, 8, 8>(g, stream);
-        if (rc) return rc;
-        if (norms) {
-            knn_shrink_rows_kernel<<<(unsigned)((c * n + 255) / 256), 256, 0, stream>>>(c, n, S, src_rows ? src_rows + c0 : nullptr, row0 + c0,
-                                                                                      norms, shrink);
-            MMREC_LAUNCH_CHECK();
-        }
-        if (dst_pos) {
-            rc = mmrec_topk_rows_f32(c, n, S, n, k, 0, ti, tv, stream);
-            if (rc) return rc;
-            knn_scatter_kernel<<<(unsigned)((c * k + 255) / 256), 256, 0, stream>>>(c, k, dst_pos + c0, ti, tv, out_idx, out_val);
-            MMREC_LAUNCH_CHECK();
-        } else {
-            rc = mmrec_topk_rows_f32(c, n, S, n, k, 0, out_idx + (row0 + c0) * k, out_val + (row0 + c0) * k, stream);
-            if (rc) return rc;
-        }
-    }
-    return MMREC_OK;
+        if (rc || !norms) return rc;
+        knn_shrink_rows_kernel<<<(unsigned)((c * n + 255) / 256), 256, 0, stream>>>(c, n, S, src_rows ? src_rows + c0 : nullptr, c0, norms, shrink);
+        MMREC_LAUNCH_CHECK();
+        return MMREC_OK;
+    });
 }
 
 }  // namespace mmrec
@@ -605,13 +574,7 @@ static int knn_topk_impl(int64_t n, const float* X, int64_t ldx, int F, int64_t 
         set_error("knn_topk: workspace %zu < %zu", ws_bytes, P.total + 1024);
         return MMREC_EWORKSPACE;
     }
-    static bool attr_done[64] = {false};
-    int dev = 0;
-    MMREC_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_done[dev]) {
-        MMREC_CUDA(cudaFuncSetAttribute(knn_pass_kernel<SHRINK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KN_SMEM));
-        if (dev >= 0 && dev < 64) attr_done[dev] = true;
-    }
+    if (int rc = set_smem_once<knn_pass_kernel<SHRINK>>((int)KN_SMEM)) return rc;
     uint32_t* header = (uint32_t*)(base + P.off_hdr);
     float* rnorm = (float*)(base + P.off_rnorm);
     const char* Xpk = base + P.off_xpk;
@@ -640,7 +603,7 @@ static int knn_topk_impl(int64_t n, const float* X, int64_t ldx, int F, int64_t 
     // shrink route: the certificate needs a finite shrink >= 0, finite norms and, with shrink 0, no zero norm (0 / 0)
     const bool shrink_exact = SHRINK && (!(shrink >= 0.f && shrink < INFINITY) || h[4] || (shrink == 0.f && h[3] == 0x7fffffffu));
     if (h[0] >= 0x7f800000u || shrink_exact) {
-        int rc = knn_exact_rows(m, rows, nullptr, 0, n, X, ldx, F, k, P, base, out_idx, out_val, stream, norms, shrink);
+        int rc = knn_exact_rows(m, rows, nullptr, n, X, ldx, F, k, P, base, out_idx, out_val, stream, norms, shrink);
         if (rc) return rc;
         g_knn_fallback_rows = m;
         return MMREC_OK;
@@ -677,15 +640,11 @@ static int knn_topk_impl(int64_t n, const float* X, int64_t ldx, int F, int64_t 
                                                                               counter, fb_rows, fb_pos, out_idx + r0 * k, out_val + r0 * k,
                                                                               norms, shrink);
         MMREC_LAUNCH_CHECK();
-        int32_t cnt = 0;
-        MMREC_CUDA(cudaMemcpyAsync(&cnt, counter, 4, cudaMemcpyDeviceToHost, stream));
-        MMREC_CUDA(cudaStreamSynchronize(stream));
-        if (cnt > 0) {
-            int rc = knn_exact_rows(cnt, fb_rows, fb_pos, 0, n, X, ldx, F, k, P, base, out_idx + r0 * k, out_val + r0 * k, stream, norms,
-                                    shrink);
-            if (rc) return rc;
-            n_fb += cnt;
-        }
+        const int64_t cnt = read_count(counter, stream);
+        if (cnt < 0) return (int)cnt;
+        int rc = knn_exact_rows(cnt, fb_rows, fb_pos, n, X, ldx, F, k, P, base, out_idx + r0 * k, out_val + r0 * k, stream, norms, shrink);
+        if (rc) return rc;
+        n_fb += cnt;
     }
     g_knn_fallback_rows = n_fb;
     return MMREC_OK;

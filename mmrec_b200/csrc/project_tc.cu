@@ -315,20 +315,9 @@ int project_tc(int64_t n_out, const int64_t* idx, const float* table, int64_t F,
     p.vec_ok = ((F & 3) == 0) && ((((uintptr_t)table) & 15) == 0);
     p.partial = partial; p.rows_padded = P.rows_padded;
     const PjSmem L = pj_smem(P.N, P.stages);
-    {   // the opt-in is per device
-        static bool attr_set[64] = {false};
-        int dev = 0;
-        MMREC_CUDA(cudaGetDevice(&dev));
-        if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            MMREC_CUDA(cudaFuncSetAttribute(project_tc_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            if (dev >= 0 && dev < 64) attr_set[dev] = true;
-        }
-    }
+    rc = set_smem_once<project_tc_kernel<64, true>, project_tc_kernel<64, false>, project_tc_kernel<128, true>,
+                       project_tc_kernel<128, false>, project_tc_kernel<256, true>, project_tc_kernel<256, false>>(227 * 1024);
+    if (rc) return rc;
     const bool fast = p.vec_ok && (F % PJ_KC) == 0;
     const unsigned grid = (unsigned)(P.n_tiles * P.n_splits);
     if (P.N == 64) {

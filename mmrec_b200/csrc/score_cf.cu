@@ -37,8 +37,8 @@
 #include <climits>
 #include <cstdio>
 #include <cstdlib>
-#include <cub/device/device_scan.cuh>
 
+#include "batch_mask.cuh"
 #include "select.cuh"
 #include "tc_common.cuh"
 
@@ -293,140 +293,13 @@ __global__ void __launch_bounds__(256) cf_pack_items_kernel(int64_t n_items, con
     cf_pack_one(t, n_items, nullptr, Ie, ldi, d, KP, header + 4, Ipk, nullptr, header);
 }
 
-// ---- mask CSR over batch rows -------------------------------------------------------------------------------------
-// The reference's evaluation loader emits the mask row-major (batch row ascending: src/utils/dataloader.py:370-391 builds
-// it user by user), so the common case is a sorted row array: the row pointers are the positions where the row
-// changes, checked as we go, one fully parallel pass.  If any block saw a descent, mask_csr_small_kernel (one CTA:
-// count in shared memory, scan, fill) redoes the job for arbitrary order; otherwise it exits at once.
-__device__ __forceinline__ void cf_mask_sorted_block(int64_t blk, int64_t nnz, const int64_t* __restrict__ rows, const int64_t* __restrict__ cols,
-                                                     int B, int64_t item_offset, int32_t* __restrict__ ptr, int32_t* __restrict__ items,
-                                                     int32_t* __restrict__ unsorted) {
-    const int64_t j = blk * (int64_t)blockDim.x + threadIdx.x;        // entry j, plus one sentinel thread j == nnz
-    int bad = 0;
-    if (j <= nnz) {
-        const int64_t rj = j < nnz ? rows[j] : (int64_t)B;
-        const int64_t rp = j > 0 ? rows[j - 1] : -1;
-        bad = j < nnz && rp > rj;
-        if (j < nnz) items[j] = (int32_t)(cols[j] - item_offset);
-        // rows (rp, rj] start at entry j (rows outside [0, B) own no pointer; clamped so that they delimit correctly)
-        const int64_t lo = rp < -1 ? -1 : (rp > B ? B : rp), hi = rj < -1 ? -1 : (rj > B ? B : rj);
-        for (int64_t r = lo + 1; r <= hi; ++r) ptr[r] = (int32_t)j;
-    }
-    bad = __syncthreads_or(bad);
-    if (threadIdx.x == 0) unsorted[blk] = bad;
-}
-
-constexpr int MC_MAX_ROWS = 8192;
-constexpr int MC_THREADS = 1024;
-__global__ void __launch_bounds__(MC_THREADS) mask_csr_small_kernel(int64_t nnz, const int64_t* __restrict__ rows,
-                                                                    const int64_t* __restrict__ cols, int B, int64_t item_offset,
-                                                                    int32_t* __restrict__ ptr, int32_t* __restrict__ items,
-                                                                    const int32_t* __restrict__ unsorted, int n_unsorted) {
-    extern __shared__ int32_t mc_sm[];                               // count / cursor [B + 1] | warp totals [32]
-    {   // runs only when the sorted pass found the rows out of order (it then left garbage behind)
-        int any = 0;
-        for (int i = threadIdx.x; i < n_unsorted; i += MC_THREADS) any |= unsorted[i];
-        if (!__syncthreads_or(any)) return;
-    }
-    int32_t* cnt = mc_sm;
-    int32_t* wtot = mc_sm + B + 1;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    for (int r = tid; r <= B; r += MC_THREADS) cnt[r] = 0;
-    __syncthreads();
-    constexpr int MC_U = 8;                                          // loads in flight per thread (the loop is latency-bound)
-    for (int64_t jb = 0; jb < nnz; jb += (int64_t)MC_U * MC_THREADS) {        // warp-uniform trip count (match / shfl below)
-        const int64_t j0 = jb + tid;
-        int64_t r[MC_U];
-#pragma unroll
-        for (int u = 0; u < MC_U; ++u) {
-            const int64_t j = j0 + (int64_t)u * MC_THREADS;
-            r[u] = j < nnz ? __ldg(rows + j) : -1;
-        }
-#pragma unroll
-        for (int u = 0; u < MC_U; ++u) {
-            // one atomic per distinct row of the warp (same-address shared atomics serialise a full round trip each)
-            const int rr = (r[u] >= 0 && r[u] < B) ? (int)r[u] : -1;
-            const unsigned peers = __match_any_sync(0xffffffffu, rr);
-            if (rr >= 0 && lane == __ffs(peers) - 1) atomicAdd(cnt + rr, __popc(peers));
-        }
-    }
-    __syncthreads();
-    // exclusive scan of cnt[0..B]: each thread owns a contiguous run of rows
-    const int per = (B + 1 + MC_THREADS - 1) / MC_THREADS;
-    const int r0 = tid * per, r1 = min(B + 1, r0 + per);
-    int local = 0;
-    for (int r = r0; r < r1; ++r) local += cnt[r];
-    int incl = local;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += v;
-    }
-    if (lane == 31) wtot[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-        int v = wtot[lane], sc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, sc, o);
-            if (lane >= o) sc += u;
-        }
-        wtot[lane] = sc - v;                                         // exclusive warp offsets
-    }
-    __syncthreads();
-    int run = wtot[wid] + incl - local;
-    for (int r = r0; r < r1; ++r) {
-        const int c = cnt[r];
-        ptr[r] = run;
-        cnt[r] = run;                                                // becomes the fill cursor
-        run += c;
-    }
-    __syncthreads();
-    for (int64_t jb = 0; jb < nnz; jb += (int64_t)MC_U * MC_THREADS) {
-        const int64_t j0 = jb + tid;
-        int64_t r[MC_U], c[MC_U];
-#pragma unroll
-        for (int u = 0; u < MC_U; ++u) {
-            const int64_t j = j0 + (int64_t)u * MC_THREADS;
-            r[u] = j < nnz ? __ldg(rows + j) : -1;
-            c[u] = j < nnz ? __ldg(cols + j) : 0;
-        }
-#pragma unroll
-        for (int u = 0; u < MC_U; ++u) {
-            const int rr = (r[u] >= 0 && r[u] < B) ? (int)r[u] : -1;
-            const unsigned peers = __match_any_sync(0xffffffffu, rr);
-            const int leader = __ffs(peers) - 1;
-            int base = 0;
-            if (rr >= 0 && lane == leader) base = atomicAdd(cnt + rr, __popc(peers));
-            base = __shfl_sync(0xffffffffu, base, leader);
-            if (rr >= 0) items[base + __popc(peers & ((1u << lane) - 1u))] = (int32_t)(c[u] - item_offset);   // order inside a row is free
-        }
-    }
-}
-// large batches / masks: global count, library scan, fill
-__global__ void mask_count_kernel(int64_t nnz, const int64_t* __restrict__ rows, int64_t B, int32_t* __restrict__ counts) {
-    int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (j < nnz && rows[j] >= 0 && rows[j] < B) atomicAdd(counts + rows[j], 1);
-}
-__global__ void mask_fill_kernel(int64_t nnz, const int64_t* __restrict__ rows, const int64_t* __restrict__ cols, int64_t B,
-                                 int64_t item_offset, const int32_t* __restrict__ ptr, int32_t* __restrict__ cursor,
-                                 int32_t* __restrict__ items) {
-    int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (j >= nnz || rows[j] < 0 || rows[j] >= B) return;
-    const int pos = ptr[rows[j]] + atomicAdd(cursor + rows[j], 1);
-    items[pos] = (int32_t)(cols[j] - item_offset);     // may fall outside [0, n_items): then it never matches
-}
-
-// One launch per row block for everything the passes need prepared: the sorted-mask CSR (first call only), the user
-// operand + row norms, and the zeroing of the flags / slot counter.
-__global__ void __launch_bounds__(256) cf_prep_kernel(int64_t mask_blocks, int64_t mask_nnz, const int64_t* __restrict__ mask_rows,
-                                                      const int64_t* __restrict__ mask_cols, int B_all, int64_t item_offset,
-                                                      int32_t* __restrict__ mptr, int32_t* __restrict__ mitems, int32_t* __restrict__ unsorted,
-                                                      int64_t nb, const int64_t* __restrict__ users, const float* __restrict__ Ue, int64_t ldu,
-                                                      int d, int KP, uint4* __restrict__ Upk, float* __restrict__ unorm, int64_t pack_threads,
-                                                      uint32_t* __restrict__ zero, int64_t zero_words) {
+// One launch per row block for everything the passes need prepared: the sorted pass of the batch mask CSR (first call
+// only, batch_mask.cuh), the user operand + row norms, and the zeroing of the flags / slot counter.
+__global__ void __launch_bounds__(256) cf_prep_kernel(int64_t mask_blocks, const BatchMask mask, int64_t nb, const int64_t* __restrict__ users,
+                                                      const float* __restrict__ Ue, int64_t ldu, int d, int KP, uint4* __restrict__ Upk,
+                                                      float* __restrict__ unorm, int64_t pack_threads, uint32_t* __restrict__ zero, int64_t zero_words) {
     if ((int64_t)blockIdx.x < mask_blocks) {
-        cf_mask_sorted_block(blockIdx.x, mask_nnz, mask_rows, mask_cols, B_all, item_offset, mptr, mitems, unsorted);
+        mask_sorted_block(blockIdx.x, mask);
         return;
     }
     int64_t t = (blockIdx.x - mask_blocks) * (int64_t)blockDim.x + threadIdx.x;
@@ -826,7 +699,7 @@ int cf_catalog_pack(int64_t n_items, const float* Ie, int64_t ldi, int d, void* 
 struct CfPlan {
     int KP, gw, G;
     int64_t n_it, rows_blk, rows_pad, n_pairs;
-    size_t off_cat, off_upk, off_unorm, off_gmax, off_thr, off_bitmap, off_flags, off_mptr, off_mcur, off_mitems, off_cub, off_keys, cub_bytes, total;
+    size_t off_cat, off_upk, off_unorm, off_gmax, off_thr, off_bitmap, off_flags, off_mask, off_keys, total;
 };
 
 static CfPlan cf_plan(int64_t B, int64_t n_items, int d, int64_t mask_nnz, bool with_cat) {
@@ -852,13 +725,7 @@ static CfPlan cf_plan(int64_t B, int64_t n_items, int d, int64_t mask_nnz, bool 
     P.off_thr = take((size_t)P.rows_pad * 4);
     P.off_bitmap = take((size_t)P.rows_blk * P.n_it * 16);
     P.off_flags = take((size_t)(2 * P.rows_blk + 2) * 4);            // flags [rows_blk] | counter | row_of_slot [rows_blk]   (flags + counter zeroed per block)
-    P.off_mptr = take((size_t)(B + 2) * 4);
-    P.off_mcur = take((size_t)(B + 2 > 1100 ? B + 2 : 1100) * 4);    // fill cursors, or the per-block order flags of the sorted-mask pass
-    P.off_mitems = take((size_t)(mask_nnz > 0 ? mask_nnz : 1) * 4);
-    size_t scan_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t*)nullptr, (int32_t*)nullptr, (int64_t)(B + 1));
-    P.cub_bytes = scan_bytes;
-    P.off_cub = take(scan_bytes);
+    P.off_mask = take(batch_mask(nullptr, mask_nnz, nullptr, nullptr, B, 0, 0).bytes);
     P.off_keys = take((size_t)CF_EX_SLOTS * n_items * 4);
     P.total = off + 1024;
     return P;
@@ -873,22 +740,6 @@ bool score_cf_supported(int64_t B, int64_t n_items, int d, int k) {
 size_t score_cf_workspace_bytes(int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, bool with_cat) {
     if (!score_cf_supported(B, n_items, d, k)) return 0;
     return cf_plan(B, n_items, d, mask_nnz, with_cat).total;
-}
-
-static int cf_set_attrs() {
-    static bool done[64] = {false};
-    int dev = 0;
-    MMREC_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !done[dev]) {                        // the attribute is per device
-        MMREC_CUDA(cudaFuncSetAttribute(cf_pass_kernel<1, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        MMREC_CUDA(cudaFuncSetAttribute(cf_pass_kernel<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        MMREC_CUDA(cudaFuncSetAttribute(cf_pass_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        MMREC_CUDA(cudaFuncSetAttribute(cf_pass_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        MMREC_CUDA(cudaFuncSetAttribute(cf_pass_kernel<2, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        MMREC_CUDA(cudaFuncSetAttribute(mask_csr_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-        if (dev >= 0 && dev < 64) done[dev] = true;
-    }
-    return MMREC_OK;
 }
 
 // Stage timing (tuning aid): with env MMREC_CF_TIMING set, the stages of the LAST score_cf call are bracketed by CUDA events
@@ -920,7 +771,8 @@ int score_cf(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int6
     const CfPlan P = cf_plan(B, n_items, d, mask_nnz, cat == nullptr);
     char* base = (char*)(((uintptr_t)ws + 1023) & ~(uintptr_t)1023);
     if (ws_bytes < P.total + (size_t)(base - (char*)ws)) return 0;
-    { int rc = cf_set_attrs(); if (rc) return rc; }
+    if (int rc = set_smem_once<cf_pass_kernel<1, 8>, cf_pass_kernel<1, 4>, cf_pass_kernel<1, 2>, cf_pass_kernel<1, 1>, cf_pass_kernel<2, 8>>(227 * 1024))
+        return rc;
     if (g_cf_timing < 0) g_cf_timing = getenv("MMREC_CF_TIMING") ? 1 : 0;
     g_cf_nev = 0;
     cf_mark(stream);                                                  // stages: pack | prep + mask | pass 1 | thr | pass 2 | final | exact
@@ -938,20 +790,14 @@ int score_cf(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int6
     int32_t* flags = (int32_t*)(base + P.off_flags);
     int32_t* counter = flags + P.rows_blk;
     int32_t* row_of_slot = counter + 1;
-    int32_t *mptr = (int32_t*)(base + P.off_mptr), *mcur = (int32_t*)(base + P.off_mcur), *mitems = (int32_t*)(base + P.off_mitems);
+    const BatchMask M = batch_mask(base + P.off_mask, mask_nnz, mask_rows, mask_cols, B, item_offset, n_items);
     unsigned* keys = (unsigned*)(base + P.off_keys);
-    const int T = 256;
+    constexpr int T = MC_SORTED_THREADS;                              // (256: cf_prep_kernel's blocks run the sorted mask pass)
     const bool has_mask = mask_nnz > 0;
-    const bool small_mask = has_mask && B <= MC_MAX_ROWS && mask_nnz <= (1ll << 18);
+    const bool small_mask = has_mask && mask_small(B, mask_nnz);
     if (has_mask && !small_mask) {
-        MMREC_CUDA(cudaMemsetAsync(mcur, 0, (size_t)(B + 2) * 4, stream));
-        mask_count_kernel<<<(unsigned)((mask_nnz + T - 1) / T), T, 0, stream>>>(mask_nnz, mask_rows, B, mcur);
-        MMREC_LAUNCH_CHECK();
-        size_t tmp = P.cub_bytes;
-        MMREC_CUDA(cub::DeviceScan::ExclusiveSum(base + P.off_cub, tmp, mcur, mptr, B + 1, stream));
-        MMREC_CUDA(cudaMemsetAsync(mcur, 0, (size_t)(B + 2) * 4, stream));
-        mask_fill_kernel<<<(unsigned)((mask_nnz + T - 1) / T), T, 0, stream>>>(mask_nnz, mask_rows, mask_cols, B, item_offset, mptr, mcur, mitems);
-        MMREC_LAUNCH_CHECK();
+        int rc = batch_mask_large(M, stream);
+        if (rc) return rc;
     }
     const CfSmem L = cf_smem(P.KP);
     const int sms = sm_count();
@@ -961,19 +807,17 @@ int score_cf(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int6
         const int64_t n_pairs = nb_pad / (2 * CF_TILE);
         const int64_t* ub = users ? users + r0 : nullptr;
         const float* ue = users ? Ue : Ue + r0 * ldu;
-        const int32_t* mp = has_mask ? mptr + r0 : nullptr;
+        const int32_t* mp = has_mask ? M.ptr + r0 : nullptr;
         // prep: [mask CSR of the whole batch (first block, sorted case)] + user operand + zeroed flags / counter
-        const int64_t mask_blocks = (small_mask && r0 == 0) ? (mask_nnz + 1 + T - 1) / T : 0;      // <= 1025 words of mcur hold the order flags
+        const int64_t mask_blocks = (small_mask && r0 == 0) ? mask_sorted_blocks(mask_nnz) : 0;
         const int64_t pack_threads = nb_pad * (P.KP / 8);
         const int64_t zero_words = P.rows_blk + 1;
         cf_prep_kernel<<<(unsigned)(mask_blocks + (pack_threads + zero_words + T - 1) / T), T, 0, stream>>>(
-            mask_blocks, mask_nnz, mask_rows, mask_cols, (int)B, item_offset, mptr, mitems, mcur, nb, ub, ue, ldu, d, P.KP, Upk, unorm,
-            pack_threads, (uint32_t*)flags, zero_words);
+            mask_blocks, M, nb, ub, ue, ldu, d, P.KP, Upk, unorm, pack_threads, (uint32_t*)flags, zero_words);
         MMREC_LAUNCH_CHECK();
         if (mask_blocks) {
-            mask_csr_small_kernel<<<1, MC_THREADS, (size_t)(B + 1 + 32) * 4, stream>>>(mask_nnz, mask_rows, mask_cols, (int)B, item_offset, mptr,
-                                                                                     mitems, mcur, (int)mask_blocks);
-            MMREC_LAUNCH_CHECK();
+            int rc = batch_mask_unsorted(M, stream);
+            if (rc) return rc;
         }
         cf_mark(stream);
         CfParams p;
@@ -998,13 +842,13 @@ int score_cf(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int6
         {
             const unsigned fg = (unsigned)((nb + CF_FIN_WARPS - 1) / CF_FIN_WARPS);
 #define CF_FINAL(LPR) cf_final_kernel<LPR><<<fg, 32 * CF_FIN_WARPS, 0, stream>>>(nb, (int)P.n_it, n_items, d, k, item_offset, bitmap, ub, ue, ldu, Ie, ldi, mp, \
-                                                                            mitems, flags, counter, row_of_slot, out_idx + r0 * k, out_val + r0 * k)
+                                                                            M.items, flags, counter, row_of_slot, out_idx + r0 * k, out_val + r0 * k)
             if (cf_lpr(d) == 8) CF_FINAL(8); else if (cf_lpr(d) == 16) CF_FINAL(16); else CF_FINAL(32);
 #undef CF_FINAL
         }
         MMREC_LAUNCH_CHECK();
         cf_mark(stream);
-        cf_exact_kernel<<<CF_EX_SLOTS, 256, 0, stream>>>(ub, ue, ldu, n_items, Ie, ldi, d, k, item_offset, mp, mitems, counter, row_of_slot, keys,
+        cf_exact_kernel<<<CF_EX_SLOTS, 256, 0, stream>>>(ub, ue, ldu, n_items, Ie, ldi, d, k, item_offset, mp, M.items, counter, row_of_slot, keys,
                                                          out_idx + r0 * k, out_val + r0 * k);
         MMREC_LAUNCH_CHECK();
         cf_mark(stream);

@@ -194,15 +194,7 @@ int score_tc(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int6
     p.tiles_per_split = (int)((n_it + splits - 1) / splits);
     p.n_splits = (int)((n_it + p.tiles_per_split - 1) / p.tiles_per_split);
     const TcSmemLayout L = tc_smem_layout(KP);
-    {   // the opt-in is per device
-        static bool attr_set[64] = {false};
-        int dev = 0;
-        MMREC_CUDA(cudaGetDevice(&dev));
-        if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-            MMREC_CUDA(cudaFuncSetAttribute(score_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            if (dev >= 0 && dev < 64) attr_set[dev] = true;
-        }
-    }
+    if (int rc = set_smem_once<score_tc_kernel>(227 * 1024)) return rc;
     score_tc_kernel<<<(unsigned)(n_ut * p.n_splits), TC_THREADS, L.total, stream>>>(p);
     MMREC_LAUNCH_CHECK();
     return 1;

@@ -16,8 +16,8 @@
 //                            (r, s) beside them in shared memory;
 //                         2. bitonic sort (select.cuh) on (column, slot): each column's products in R order;
 //                         3. one thread per column sums its products in that order -- the same fmaf chain as the dense row;
-//                         4. the row's masked items (batch mask CSR) are sorted; each is looked up by binary search among
-//                            the summed columns;
+//                         4. the row's masked items (batch mask CSR, batch_mask.cuh) are sorted; each is looked up by binary
+//                            search among the summed columns;
 //                         5. rank.  The dense row is +0.0 everywhere except at the "exceptions": masked items (-1e10) and
 //                            unmasked columns whose sum is not +0.0 (bit pattern).  The exceptions are sorted on (float_key,
 //                            ~index); the output is the exceptions above +0.0, then the +0.0 items in ascending index
@@ -26,8 +26,10 @@
 //                         the dense row after mmrec_mask_f32: -0.0 sorts below +0.0, masked items are -1e10, and k beyond
 //                         the unmasked items runs into them.
 //   exact route           rows with more than SP_CAP products, more than SP_MCAP masked items or a non-finite sum are listed;
-//                         the host then runs the unfused route on them -- the same row kernel, the same mask value,
-//                         mmrec_topk_rows_f32 -- and scatters the results.  Bit-identical by construction.
+//                         the host then runs the unfused route on them (exact_rows.cuh) -- the same row kernel, the same mask
+//                         value, mmrec_topk_rows_f32 -- and scatters the results.  Bit-identical by construction.
+#include "batch_mask.cuh"
+#include "exact_rows.cuh"
 #include "select.cuh"
 
 namespace mmrec {
@@ -65,54 +67,6 @@ __global__ void __launch_bounds__(256) sparse_scores_kernel(int64_t nb, const in
     if (j >= nb) return;
     const int64_t b = pos ? pos[j] : j;
     sparse_score_row(users ? users[b] : b, R, S, out + j * ldo, threadIdx.x & 31);
-}
-
-// ---- batch mask CSR (rows outside [0, B) and items outside [0, n_items) are dropped later, as mmrec_mask_f32 ignores them)
-__global__ void sp_mask_count_kernel(int64_t nnz, const int64_t* __restrict__ rows, int64_t B, int32_t* __restrict__ cnt) {
-    const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (j < nnz && rows[j] >= 0 && rows[j] < B) atomicAdd(cnt + rows[j], 1);
-}
-
-// in-place exclusive scan of a[0 .. n), one CTA of 1024 threads (each owns a contiguous run)
-__global__ void __launch_bounds__(1024) sp_scan_kernel(int64_t n, int32_t* __restrict__ a) {
-    __shared__ int32_t wtot[32];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int64_t per = (n + 1023) / 1024, r0 = tid * per, r1 = r0 + per < n ? r0 + per : n;
-    int local = 0;
-    for (int64_t r = r0; r < r1; ++r) local += a[r];
-    int incl = local;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += v;
-    }
-    if (lane == 31) wtot[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-        const int v = wtot[lane];
-        int sc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int w = __shfl_up_sync(0xffffffffu, sc, o);
-            if (lane >= o) sc += w;
-        }
-        wtot[lane] = sc - v;
-    }
-    __syncthreads();
-    int run = wtot[wid] + incl - local;
-    for (int64_t r = r0; r < r1; ++r) {
-        const int c = a[r];
-        a[r] = run;
-        run += c;
-    }
-}
-
-__global__ void sp_mask_fill_kernel(int64_t nnz, const int64_t* __restrict__ rows, const int64_t* __restrict__ cols, int64_t B,
-                                    const int32_t* __restrict__ ptr, int32_t* __restrict__ cursor, int32_t* __restrict__ items) {
-    const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (j >= nnz || rows[j] < 0 || rows[j] >= B) return;
-    const int64_t c = cols[j];
-    items[ptr[rows[j]] + atomicAdd(cursor + rows[j], 1)] = (c >= 0 && c < (1ll << 31)) ? (int32_t)c : -1;   // (-1: never matches)
 }
 
 // ---- the fused row -------------------------------------------------------------------------------------------------
@@ -310,38 +264,21 @@ __global__ void sp_mask_rows_kernel(int64_t c, const int64_t* __restrict__ pos, 
     }
 }
 
-__global__ void sp_scatter_kernel(int64_t c, int k, const int64_t* __restrict__ pos, const int64_t* __restrict__ ti, const float* __restrict__ tv,
-                                  int64_t* __restrict__ out_idx, float* __restrict__ out_val) {
-    const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (t >= c * k) return;
-    const int64_t s = t / k, j = t - s * k;
-    out_idx[pos[s] * k + j] = ti[t];
-    out_val[pos[s] * k + j] = tv[t];
-}
-
 // ---- host side ------------------------------------------------------------------------------------------------------
 struct SpPlan {
     int64_t s_rows;
-    size_t off_mptr, off_mcur, off_mitems, off_cnt, off_fb, off_s, off_ti, off_tv, total;
+    size_t off_mask, off_cnt, off_fb, off_ex, total;
 };
 
 static SpPlan sp_plan(int64_t B, int64_t n_items, int64_t mask_nnz, int k) {
     SpPlan P;
-    int64_t sr = (256ll << 20) / (4 * n_items);                       // dense block of the exact route: <= 256 MB, <= 1024 rows
-    if (sr < 1) sr = 1;
-    if (sr > 1024) sr = 1024;
-    if (sr > B) sr = B > 0 ? B : 1;
-    P.s_rows = sr;
+    P.s_rows = exact_block_rows(n_items, B > 0 ? B : 1);
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes > 0 ? bytes : 1, 256); return o; };
-    P.off_mptr = take((size_t)(B + 1) * 4);
-    P.off_mcur = take((size_t)(B + 1) * 4);
-    P.off_mitems = take((size_t)(mask_nnz > 0 ? mask_nnz : 1) * 4);
+    P.off_mask = take(batch_mask(nullptr, mask_nnz, nullptr, nullptr, B, 0, 0).bytes);
     P.off_cnt = take(4);
     P.off_fb = take((size_t)B * 8);
-    P.off_s = take((size_t)P.s_rows * n_items * 4);
-    P.off_ti = take((size_t)P.s_rows * k * 8);
-    P.off_tv = take((size_t)P.s_rows * k * 4);
+    P.off_ex = take(exact_rows_bytes(P.s_rows, n_items, k));
     P.total = off + 256;
     return P;
 }
@@ -394,53 +331,29 @@ extern "C" int mmrec_sparse_score_topk_f32(int64_t B, const int64_t* users, int6
         set_error("sparse_score_topk: workspace %zu < %zu", ws_bytes, P.total);
         return MMREC_EWORKSPACE;
     }
-    int32_t* mptr = (int32_t*)(base + P.off_mptr);
-    int32_t* mcur = (int32_t*)(base + P.off_mcur);
-    int32_t* mitems = (int32_t*)(base + P.off_mitems);
+    const BatchMask M = batch_mask(base + P.off_mask, mask_nnz, mask_rows, mask_cols, B, 0, n_items);
     int32_t* counter = (int32_t*)(base + P.off_cnt);
     int64_t* fb = (int64_t*)(base + P.off_fb);
     const SpCsr R{r_ptr, r_col, r_val}, S{s_ptr, s_col, s_val};
     if (mask_nnz > 0) {
-        MMREC_CUDA(cudaMemsetAsync(mptr, 0, (size_t)(B + 1) * 4, stream));
-        MMREC_CUDA(cudaMemsetAsync(mcur, 0, (size_t)(B + 1) * 4, stream));
-        const unsigned g = (unsigned)((mask_nnz + 255) / 256);
-        sp_mask_count_kernel<<<g, 256, 0, stream>>>(mask_nnz, mask_rows, B, mptr);
-        MMREC_LAUNCH_CHECK();
-        sp_scan_kernel<<<1, 1024, 0, stream>>>(B + 1, mptr);
-        MMREC_LAUNCH_CHECK();
-        sp_mask_fill_kernel<<<g, 256, 0, stream>>>(mask_nnz, mask_rows, mask_cols, B, mptr, mcur, mitems);
-        MMREC_LAUNCH_CHECK();
+        int rc = batch_mask_build(M, stream);
+        if (rc) return rc;
     }
-    const int32_t* mp = mask_nnz > 0 ? mptr : nullptr;
-    static bool attr_done[64] = {false};
-    int dev = 0;
-    MMREC_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_done[dev]) {
-        MMREC_CUDA(cudaFuncSetAttribute(sparse_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SP_SMEM));
-        if (dev >= 0 && dev < 64) attr_done[dev] = true;
-    }
+    const int32_t* mp = mask_nnz > 0 ? M.ptr : nullptr;
+    if (int rc = set_smem_once<sparse_topk_kernel>((int)SP_SMEM)) return rc;
     MMREC_CUDA(cudaMemsetAsync(counter, 0, 4, stream));
-    sparse_topk_kernel<<<(unsigned)B, SP_THREADS, SP_SMEM, stream>>>(n_items, users, R, S, mp, mitems, k, counter, fb, out_idx, out_val);
+    sparse_topk_kernel<<<(unsigned)B, SP_THREADS, SP_SMEM, stream>>>(n_items, users, R, S, mp, M.items, k, counter, fb, out_idx, out_val);
     MMREC_LAUNCH_CHECK();
-    int32_t cnt = 0;
-    MMREC_CUDA(cudaMemcpyAsync(&cnt, counter, 4, cudaMemcpyDeviceToHost, stream));
-    MMREC_CUDA(cudaStreamSynchronize(stream));
-    float* Sd = (float*)(base + P.off_s);
-    int64_t* ti = (int64_t*)(base + P.off_ti);
-    float* tv = (float*)(base + P.off_tv);
-    for (int64_t c0 = 0; c0 < cnt; c0 += P.s_rows) {
-        const int64_t c = cnt - c0 < P.s_rows ? cnt - c0 : P.s_rows;
-        int rc = sp_scores_rows(c, users, fb + c0, R, S, n_items, Sd, n_items, stream);
-        if (rc) return rc;
-        if (mp) {
-            sp_mask_rows_kernel<<<(unsigned)c, 256, 0, stream>>>(c, fb + c0, mp, mitems, n_items, Sd);
-            MMREC_LAUNCH_CHECK();
-        }
-        rc = mmrec_topk_rows_f32(c, n_items, Sd, n_items, k, 0, ti, tv, stream);
-        if (rc) return rc;
-        sp_scatter_kernel<<<(unsigned)((c * k + 255) / 256), 256, 0, stream>>>(c, k, fb + c0, ti, tv, out_idx, out_val);
+    const int64_t cnt = read_count(counter, stream);
+    if (cnt < 0) return (int)cnt;
+    int rc = exact_rows_topk(cnt, fb, n_items, k, P.s_rows, base + P.off_ex, out_idx, out_val, stream, [&](int64_t c0, int64_t c, float* Sd) {
+        int rc2 = sp_scores_rows(c, users, fb + c0, R, S, n_items, Sd, n_items, stream);
+        if (rc2 || !mp) return rc2;
+        sp_mask_rows_kernel<<<(unsigned)c, 256, 0, stream>>>(c, fb + c0, mp, M.items, n_items, Sd);
         MMREC_LAUNCH_CHECK();
-    }
+        return MMREC_OK;
+    });
+    if (rc) return rc;
     g_sparse_topk_fallback_rows = cnt;
     return MMREC_OK;
 }

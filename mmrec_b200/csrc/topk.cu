@@ -1,4 +1,5 @@
-// K3 (part): train-positive mask, exact per-row top-k, and the cross-shard top-k merge.
+// K3 (part): train-positive mask, exact per-row top-k, the cross-shard top-k merge, and the scatter of the exact route on
+// listed rows (exact_rows.cuh).
 // Contract (stronger than torch.topk, which leaves tie order open): descending value, equal values in
 // ascending item index.  Replaces src/common/trainer.py:307-309.
 //
@@ -7,6 +8,7 @@
 // k-th key are taken in index order (block-wide ordered compaction), then a bitonic sort on the composite
 // (key, ~index) puts the k winners in contract order.  (A warp-per-row streaming filter with bitonic compaction
 // was measured 2.5x slower at 7k items: the compaction sorts dominate.)
+#include "exact_rows.cuh"
 #include "peer_sync.cuh"
 #include "select.cuh"
 
@@ -144,6 +146,15 @@ int mask_apply(int64_t mask_nnz, const int64_t* mask_rows, const int64_t* mask_c
                                                                         item_offset, S, ldS);
     MMREC_LAUNCH_CHECK();
     return MMREC_OK;
+}
+
+__global__ void exact_scatter_kernel(int64_t c, int k, const int64_t* __restrict__ pos, const int64_t* __restrict__ ti,
+                                     const float* __restrict__ tv, int64_t* __restrict__ out_idx, float* __restrict__ out_val) {
+    const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (t >= c * k) return;
+    const int64_t s = t / k, j = t - s * k;
+    out_idx[pos[s] * k + j] = ti[t];
+    out_val[pos[s] * k + j] = tv[t];
 }
 }  // namespace mmrec
 

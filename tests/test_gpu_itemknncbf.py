@@ -178,6 +178,26 @@ def test_sparse_score_topk_equals_scores_plus_mask_topk(k, unit):
     assert torch.equal(idx, ei) and torch.equal(_bits(val), _bits(ev))
 
 
+@pytest.mark.parametrize("route", ["sorted", "unsorted", "large"])
+def test_sparse_score_topk_mask_routes_and_wrapping_columns(route):
+    """Each route of the batch mask CSR (rows in order, out of order, B > 8192), with a column 2^32 + j per row, j the
+    row's unmasked top-1: mmrec_mask_f32 ignores such a column although its low 32 bits name item j, and so must K9."""
+    from mmrec_b200 import ops
+    dev = _dev()
+    (rows, cols, rv, sv, si), R, S = _graphs(600, 4000, 10, seed=7)
+    users = np.arange(9000 if route == "large" else 600, dtype=np.int64) % 600
+    tu, tm = torch.from_numpy(users).to(dev), torch.from_numpy(_mask_for(users, rows, cols)).to(dev)
+    sc = ops.sparse_scores(R, S, tu)
+    _, top = ops.mask_topk(sc.clone(), tm, 1)
+    m = torch.cat([tm, torch.stack([torch.arange(len(users), device=dev), top[:, 0] + 2 ** 32])], 1)
+    order = torch.randperm(m.shape[1]) if route == "unsorted" else torch.argsort(m[0].cpu(), stable=True)
+    m = m[:, order.to(dev)]
+    val, idx = ops.sparse_score_topk(R, S, tu, m, 20)
+    assert ops.sparse_topk_fallback_rows() == 0
+    ev, ei = ops.mask_topk(sc.clone(), m, 20)
+    assert torch.equal(idx, ei) and torch.equal(_bits(val), _bits(ev))
+
+
 def test_sparse_score_topk_ranking_cases():
     """Few candidates (the +0.0 class fills the rest, masked items skipped), negative sums, a -0.0 sum, k beyond the
     unmasked items (the -1e10 entries follow), and a history whose products overflow shared memory (the unfused route)."""

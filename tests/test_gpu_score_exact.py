@@ -249,6 +249,29 @@ def test_exact_masks(dev):
     check(ue, ie, users, ms, k, item_offset=off, fallback=need_rows(ms, B, k, G_valid), what="item_offset")
 
 
+@pytest.mark.parametrize("route", ["sorted", "unsorted", "large"])
+def test_mask_columns_wrapping_32_bits(dev, route):
+    """Mask columns item_offset + 2^32 + j and item_offset - 2^32 + j lie outside the shard, so ops.mask_topk ignores
+    them, although their low 32 bits name item j -- here the first and second of the row's unmasked top-k.  The fused
+    call must ignore them too (they still count in need), whichever route builds the mask CSR: rows in order, out of
+    order, or B > 8192.  Quantised values: the unfused scores are exact, the same bits as the fused chain."""
+    from mmrec_b200 import ops
+    B = 9000 if route == "large" else 300
+    I, d, k, off = 3000, 32, 20, 1000
+    g = torch.Generator().manual_seed(41)
+    ue = (torch.randint(-16, 17, (B, d), generator=g).float() / 64).to(dev)
+    ie = (torch.randint(-16, 17, (I, d), generator=g).float() / 64).to(dev)
+    mask = torch.stack([torch.randint(0, B, (B * 4,), generator=g), torch.randint(0, I, (B * 4,), generator=g) + off]).to(dev)
+    _, top = ops.mask_topk(ops.score(ue, ie), mask, 2, off)
+    wrap = torch.stack([torch.arange(B, device=dev).repeat(2), torch.cat([top[:, 0] + 2 ** 32, top[:, 1] - 2 ** 32])])
+    m = torch.cat([mask, wrap], 1)
+    order = torch.randperm(m.shape[1], generator=g) if route == "unsorted" else torch.argsort(m[0].cpu(), stable=True)
+    m = m[:, order.to(dev)]
+    v, i, _ = check(ue, ie, None, m, k, item_offset=off, fallback=lambda fb: fb <= B // 8, what=route)
+    rv, ri = ops.mask_topk(ops.score(ue, ie), m, k, off)
+    assert torch.equal(i, ri) and torch.equal(bits(v), bits(rv))
+
+
 # ------------------------------------------------------------------------------------------------ adversarial values
 def test_exact_quantised_ties(dev):
     """Multiples of 2^-6: exact scores and exact ties at the k boundary, ranked by the tie pass of cf_final_kernel."""
