@@ -241,6 +241,15 @@ int mmrec_score_topk_cat_f32(int64_t B, const int64_t* users, const float* Ue, i
 /* diagnostic, synchronising: rows of the last row block of the last fused call on `ws` that needed the exact kernel
  * (with_cat: the call packed its catalogue into ws, i.e. cat was NULL) */
 int64_t mmrec_debug_fused_fallback_rows(const void* ws, int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, int with_cat);
+/* diagnostic, host only (no launch, no synchronisation): the scratch layout of a fused call with these arguments, for
+ * reading the filter's intermediate stages back after the call.  Fills out[0 .. min(cap, 16) - 1] with
+ *   rows_blk, rows_pad, KP, gw, n_it, G, G_valid,
+ *   catalogue offset (-1 when with_cat == 0: the catalogue lives in the caller's buffer), catalogue header bytes (the
+ *   fp16 item tiles follow the header), user pack, user row norms, gmax [rows_blk][G], thr, bitmap [rows_blk][n_it] x
+ *   16 B, flags [rows_blk] | counter | row_of_slot, total workspace,
+ * offsets in bytes from the workspace pointer rounded up to 1024.  Only the last row block's scratch survives a call.
+ * Returns the number of entries (16), -1 for a shape the fused path does not take. */
+int mmrec_debug_cf_scratch(int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, int with_cat, int64_t* out, int cap);
 /* tuning aid: with env MMREC_CF_TIMING set, device time in microseconds of the stages of the last fused call (host array
  * us[cap]; stages: catalogue pack | prep + mask | pass 1 | threshold | pass 2 | finalists | exact rows); returns the count */
 int mmrec_debug_cf_timing(float* us, int cap);
@@ -268,6 +277,14 @@ size_t mmrec_knn_topk_workspace_bytes(int64_t n, int F, int64_t m, int k);
 int mmrec_knn_topk_f32(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k,
                        int64_t* out_idx, float* out_val, void* ws, size_t ws_bytes, void* stream);
 int64_t mmrec_debug_knn_fallback_rows(void);
+/* diagnostic, host only (no launch, no synchronisation): the scratch layout of mmrec_knn_topk_f32 / _shrink_f32 with
+ * these arguments.  Fills out[0 .. min(cap, 15) - 1] with
+ *   rows_blk, rows_pad, KP, items per group (16), n_it, G, G_valid,
+ *   header (words: [0] largest |element| bits, [1] largest row norm bits; shrink route [2] .. [5]), fp16 item tiles,
+ *   row norms [n], query pack, gmax [rows_blk][G], thr, flags, total workspace,
+ * offsets in bytes from the workspace pointer rounded up to 1024.  Only the last row block's scratch survives a call.
+ * Returns the number of entries (15), -1 for arguments mmrec_knn_topk_workspace_bytes refuses. */
+int mmrec_debug_knn_scratch(int64_t n, int F, int64_t m, int k, int64_t* out, int cap);
 /* mmrec_knn_topk_shrink_f32: the same, ranked by the shrunk similarity of ItemKNNCBF's `build_item_sim_matrix`
  *                     (src/models/itemknncbf.py:56-65): v(q, i) = s(q, i) / ((norms[q] * norms[i]) + shrink), s the exact
  *                     chain above, the denominator two IEEE fp32 roundings (multiply, then add) and an IEEE division.

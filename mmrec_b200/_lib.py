@@ -51,9 +51,11 @@ PROTOTYPES = {
                                         _sz, _p]),
     "mmrec_debug_cf_timing": (_i32, [_p, _i32]),
     "mmrec_debug_fused_fallback_rows": (_i64, [_p, _i64, _i64, _i32, _i32, _i64, _i32]),
+    "mmrec_debug_cf_scratch": (_i32, [_i64, _i64, _i32, _i32, _i64, _i32, _p, _i32]),
     "mmrec_knn_topk_workspace_bytes": (_sz, [_i64, _i32, _i64, _i32]),
     "mmrec_knn_topk_f32": (_i32, [_i64, _p, _i64, _i32, _i64, _p, _i32, _p, _p, _p, _sz, _p]),
     "mmrec_debug_knn_fallback_rows": (_i64, []),
+    "mmrec_debug_knn_scratch": (_i32, [_i64, _i32, _i64, _i32, _p, _i32]),
     "mmrec_knn_topk_shrink_f32": (_i32, [_i64, _p, _i64, _i32, _i64, _p, _i32, _p, _f32, _p, _p, _p, _sz, _p]),
     "mmrec_sparse_scores_f32": (_i32, [_i64, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _i64, _p]),
     "mmrec_sparse_score_topk_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32]),

@@ -36,16 +36,21 @@
 //       |a^ . b^ - s*| <= (2^-10 + 2^-22) |a| |b| + 2^-25 sqrt(F) (|a| + |b|) + F 2^-50                 (Cauchy-Schwarz);
 //       the products a^_k b^_k (11 x 11 significand bits) are exact in fp32.
 //   (2) tensor-core accumulation over S = F_pad / 16 MMA steps.  ASSUMPTION about the hardware: one m64n128k16 step adds its
-//       16 exact products to the fp32 accumulator c with an error of at most 2^-22 (|c| + sum_j |p_j|) -- two fp32 ulps of
-//       the magnitude sum, which covers an adder that aligns to the largest exponent and truncates (one ulp) with a factor
-//       of two to spare (published measurements of Volta..Hopper tensor cores find truncation with a few guard bits, not
-//       more error).  Summed over the steps, with |c_s| <= sum of the earlier |p| (1 + small):
-//       |s~ - a^ . b^| <= S 2^-22 (1 + 2^-10) sum_k |a^_k b^_k| <= S 2^-22 (1 + 2^-9) |a| |b|.
+//       16 exact products to the fp32 accumulator c with an error of at most 2^-20 (|c| + sum_j |p_j|) -- eight fp32 ulps
+//       of the magnitude sum.  The H100 adder, as measured on an H100 SXM (tests/test_gpu_filter_stages.py: one product
+//       2^28 at the bottom of its binade beside 3 / 7 / 15 products just below 2^(5 - g), g = 0 .. 3, and the same after a
+//       large accumulator; reproduced exactly by the model in tests/test_filter_stages_host.py): every addend (c and the
+//       16 products) is aligned to the largest one's exponent and truncated 2 bits below its ulp, the aligned sum is
+//       exact and is then truncated to 24 bits.  So the 16 smaller addends lose < 16 x ulp / 4 and the final truncation
+//       < one ulp of the result: < 5 x 2^-23 (|c| + sum |p|) = 2.5 x 2^-22; the worst measured is 2.25 x 2^-22 (15
+//       products just below ulp / 2).  2^-20 leaves a factor 1.6 on the model.  Summed over the steps, with
+//       |c_s| <= sum of the earlier |p| (1 + small):
+//       |s~ - a^ . b^| <= S 2^-20 (1 + 2^-10) sum_k |a^_k b^_k| <= S 2^-20 (1 + 2^-9) |a| |b|.
 //   (3) the exact value itself is an fp32 chain of F fmaf: |s - s*| <= gamma_F sum |a_k b_k|, gamma_F = F 2^-24 / (1 - F 2^-24)
 //       (<= F 2^-24 (1 + 2^-9) for F <= 2^15; longer rows only make the margin larger through the formula below).
-//   Hence |s~ - s| <= eps(F) |a| |b| + sub(F),  eps(F) = 2^-10 + 2^-22 + (S 2^-22 + F 2^-24)(1 + 2^-9),
+//   Hence |s~ - s| <= eps(F) |a| |b| + sub(F),  eps(F) = 2^-10 + 2^-22 + (S 2^-20 + F 2^-24)(1 + 2^-9),
 //   sub(F) = 2^-25 sqrt(F) (|a| + |b|) + F 2^-50 + F 2^-149 sc^2 (subnormal steps of the unscaled chain).
-//   At F = 4096: eps = 9.77e-4 + 6.1e-5 + 2.44e-4 = 1.28e-3.  eps' (per query row) uses |a| = the row's norm and max|b| =
+//   At F = 4096: eps = 9.77e-4 + 2.44e-4 + 2.44e-4 = 1.47e-3.  eps' (per query row) uses |a| = the row's norm and max|b| =
 //   the largest row norm, both rounded up; the margin is 2 eps' inflated by 2^-8 for the rounding of its own arithmetic.
 // CERTIFICATE: at least k groups have a maximum >= t, so at least k distinct items have s~ >= t and s >= t - eps'; the k-th
 // largest exact value s_k is >= t - eps'.  Every member of the true top-k and every item tied with s_k has s >= s_k, so its
@@ -338,7 +343,7 @@ __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int
         const float RR = __fmul_ru(__fmul_ru(A == 0.f ? 0.f : __fdiv_ru(A, nq), Rmax), fac) * (1.0f + 0x1p-20f);
         const float Dmin = __fmul_rd(__fadd_rd(__fmul_rd(nq, nmin), shrink), 1.0f - 0x1p-22f);
         const float steps = (float)((F + KN_KC - 1) / KN_KC * (KN_KC / 16));
-        const float eps = 0x1p-10f + 0x1p-22f + (steps * 0x1p-22f + (float)F * 0x1p-24f) * (1.0f + 0x1p-9f);
+        const float eps = 0x1p-10f + 0x1p-22f + (steps * 0x1p-20f + (float)F * 0x1p-24f) * (1.0f + 0x1p-9f);
         const float sub = (0x1p-25f * sqrtf((float)F) * (A + Bm) * isc + (float)F * 0x1p-50f * isc * isc + 0x1p-120f) / Dmin;
         const float vmax = RR * (1.0f + 2.0f * eps) + sub;
         set_threshold(key_float(prefix), 2.0f * (eps * RR + sub + 0x1p-23f * vmax) * (1.0f + 0x1p-8f), thr + row, flags + row);
@@ -348,7 +353,7 @@ __global__ void __launch_bounds__(256) knn_thr_kernel(int64_t nb, int64_t G, int
         const int64_t qrow = rows ? rows[row] : row_off + row;
         const float un = rnorm[qrow] * sc, mn = __uint_as_float(header[1]) * sc;
         const float steps = (float)((F + KN_KC - 1) / KN_KC * (KN_KC / 16));
-        const float eps = 0x1p-10f + 0x1p-22f + (steps * 0x1p-22f + (float)F * 0x1p-24f) * (1.0f + 0x1p-9f);
+        const float eps = 0x1p-10f + 0x1p-22f + (steps * 0x1p-20f + (float)F * 0x1p-24f) * (1.0f + 0x1p-9f);
         const float sub = 0x1p-25f * sqrtf((float)F) * (un + mn) + (float)F * 0x1p-50f + ((float)F * 0x1p-75f * sc) * (0x1p-74f * sc);
         set_threshold(key_float(prefix), 2.0f * (eps * un * mn + sub) * (1.0f + 0x1p-8f), thr + row, flags + row);
     }
@@ -542,6 +547,18 @@ extern "C" size_t mmrec_knn_topk_workspace_bytes(int64_t n, int F, int64_t m, in
 }
 
 extern "C" int64_t mmrec_debug_knn_fallback_rows(void) { return g_knn_fallback_rows; }
+
+extern "C" int mmrec_debug_knn_scratch(int64_t n, int F, int64_t m, int k, int64_t* out, int cap) {
+    MMREC_CHECK_ARG(out != nullptr || cap <= 0, "debug_knn_scratch: null output");
+    if (!mmrec_knn_topk_workspace_bytes(n, F, m, k)) return -1;
+    const KnnPlan P = knn_plan(n, F, m > 0 ? m : 1, k);
+    const int64_t v[] = {P.rows_blk, P.rows_pad, P.KP, KN_GROUP, P.n_it, P.G, P.G_valid, (int64_t)P.off_hdr, (int64_t)P.off_xpk,
+                         (int64_t)P.off_rnorm, (int64_t)P.off_qpk, (int64_t)P.off_gmax, (int64_t)P.off_thr, (int64_t)P.off_flags,
+                         (int64_t)P.total};
+    const int cnt = (int)(sizeof(v) / sizeof(v[0]));
+    for (int i = 0; i < cnt && i < cap; ++i) out[i] = v[i];
+    return cnt;
+}
 
 template <bool SHRINK>
 static int knn_topk_impl(int64_t n, const float* X, int64_t ldx, int F, int64_t m, const int64_t* rows, int k, const float* norms,

@@ -27,6 +27,7 @@ size_t cf_catalog_bytes(int64_t n_items, int d);
 int cf_catalog_pack(int64_t n_items, const float* Ie, int64_t ldi, int d, void* cat, size_t cat_bytes, cudaStream_t stream);
 int score_cf_timing(float* us, int cap);
 int64_t score_cf_fallback_rows(const void* ws, int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, bool with_cat);
+int score_cf_scratch(int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, bool with_cat, int64_t* out, int cap);
 
 int mask_apply(int64_t mask_nnz, const int64_t* mask_rows, const int64_t* mask_cols, int64_t row0, int64_t B,
                int64_t n_items, int64_t item_offset, float* S, int64_t ldS, cudaStream_t stream);
@@ -103,6 +104,11 @@ extern "C" int mmrec_debug_cf_timing(float* us, int cap) { return score_cf_timin
 
 extern "C" int64_t mmrec_debug_fused_fallback_rows(const void* ws, int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, int with_cat) {
     return score_cf_fallback_rows(ws, B, n_items, d, k, mask_nnz, with_cat != 0);
+}
+
+extern "C" int mmrec_debug_cf_scratch(int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, int with_cat, int64_t* out, int cap) {
+    MMREC_CHECK_ARG(out != nullptr || cap <= 0, "debug_cf_scratch: null output");
+    return score_cf_scratch(B, n_items, d, k, mask_nnz, with_cat != 0, out, cap);
 }
 
 extern "C" int mmrec_score_topk_f32(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int64_t n_items,

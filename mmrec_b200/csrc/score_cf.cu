@@ -53,7 +53,7 @@ constexpr int CF_THREADS = 32 * CF_CONSUMER_WARPS + 32;
 constexpr int CF_MAX_STAGES = 10;
 constexpr int CF_CAP = 512;                     // candidates one warp ranks per row
 constexpr int CF_EX_SLOTS = 128;                // CTAs (and key buffers) of the exact kernel
-constexpr float CF_EPS = 1.125f / 1024.f;       // |s~ - s| <= CF_EPS |u| |i|: two RN roundings to 11 significand bits (2^-11 each) + accumulation slack
+constexpr float CF_EPS = 1.125f / 1024.f;       // |s~ - s| <= CF_EPS |u| |i|: two RN roundings to 11 significand bits (2^-11 each) + slack 2^-13 for the accumulation (<= 8 steps of 2^-20, knn_cf.cu (2)) and the fp32 chain
 constexpr float CF_EPS_SUB = 1.0f / 16777216.f; // fp16 subnormal spacing 2^-24 (scaled domain): |dx| <= 2^-11 |x| + 2^-25 per element
 
 struct CfSmem {
@@ -854,6 +854,19 @@ int score_cf(int64_t B, const int64_t* users, const float* Ue, int64_t ldu, int6
         cf_mark(stream);
     }
     return 1;
+}
+
+// The scratch layout of a call with these arguments (diagnostic, host only): the dimensions and byte offsets from the
+// 1024-aligned workspace base that mmrec_debug_cf_scratch documents.  Returns the number of entries, -1 = not fused.
+int score_cf_scratch(int64_t B, int64_t n_items, int d, int k, int64_t mask_nnz, bool with_cat, int64_t* out, int cap) {
+    if (!score_cf_supported(B, n_items, d, k)) return -1;
+    const CfPlan P = cf_plan(B, n_items, d, mask_nnz, with_cat);
+    const int64_t v[] = {P.rows_blk, P.rows_pad, P.KP, P.gw, P.n_it, P.G, (n_items + 16 * P.gw - 1) / (16 * P.gw),
+                         with_cat ? (int64_t)P.off_cat : -1, (int64_t)CF_CAT_HEADER, (int64_t)P.off_upk, (int64_t)P.off_unorm,
+                         (int64_t)P.off_gmax, (int64_t)P.off_thr, (int64_t)P.off_bitmap, (int64_t)P.off_flags, (int64_t)P.total};
+    const int n = (int)(sizeof(v) / sizeof(v[0]));
+    for (int i = 0; i < n && i < cap; ++i) out[i] = v[i];
+    return n;
 }
 
 // rows of the last row block that went to the exact kernel (synchronises; diagnostic)
