@@ -123,6 +123,31 @@ int mmrec_spmm_acc_f32(int64_t n_rows, int64_t n_cols, int d,
                        const float* X, int64_t ldx, float* Y, int64_t ldy,
                        const float* acc_in, float* acc_out, int64_t ldacc, float acc_div, int y_accumulate, void* stream);
 
+/* mmrec_spmm_f32 (no gate) over the entries of the CSR whose keep bit is set, each weighted fl(vals[e] * scale):
+ * `torch.sparse.mm(sparse_dropout(A, rate), X)` of src/common/encoders.py:77-88,99 without building the dropped matrix.
+ * keep_bits uint32[ceil(nnz / 32)], bit e (word e / 32, bit e % 32) for CSR position e (mmrec_edge_keep_bits).  A dropped
+ * entry loads nothing and adds nothing; the plan, split rows, segment-order reduction and epilogues are mmrec_spmm_f32's,
+ * so the result equals mmrec_spmm_f32 on the compacted matrix with the values fl(v * scale), up to the position of the
+ * segment boundaries of split rows.  d in {32, 64, 128, 256}, 16-byte aligned operands, else MMREC_EUNSUPPORTED. */
+int mmrec_spmm_drop_f32(int64_t n_rows, int64_t n_cols, int d,
+                        const int32_t* rowptr, const int32_t* colidx, const float* vals,
+                        const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks, const int32_t* split_rows,
+                        int32_t* counters, float* partial,
+                        const float* X, int64_t ldx, float* Y, int64_t ldy,
+                        const float* acc_in, float* acc_out, int64_t ldacc, float acc_div,
+                        const uint32_t* keep_bits, float scale, void* stream);
+
+/* The keep bits of one `sparse_dropout` draw (src/common/encoders.py:77-88): draw j of `torch.rand(nnz)` belongs to the
+ * reference's j-th stored entry, which is CSR position e with draw_of[e] = j.  Position e is kept iff
+ * floorf(keep_prob + draws[draw_of[e]]) != 0, one IEEE fp32 add (keep_prob = float32(1 - rate), as torch adds it).
+ *   keep_bits   uint32[ceil(nnz / 32)]  the forward's bits, CSR order (mmrec_spmm_drop_f32)
+ *   mirror      int32[nnz] (nullable)   position of (c, r) for the entry (r, c) of a structurally symmetric CSR
+ *   keep_bits_t uint32[ceil(nnz / 32)]  (nullable, needs mirror) bit e = bit mirror[e] of keep_bits: the dropped matrix's
+ *                                       transpose on the same CSR when its values are symmetric (the backward)
+ * Bits past nnz in the last word are 0. */
+int mmrec_edge_keep_bits(int64_t nnz, const float* draws, float keep_prob, const int32_t* draw_of, const int32_t* mirror,
+                         uint32_t* keep_bits, uint32_t* keep_bits_t, void* stream);
+
 /* The SpMMs of one propagation as ONE persistent cooperative launch (src/models/freedom.py:164-178: n_ui_layers products with
  * A_hat, the item-item product, the layer mean and `+ h`): the steps run in order on one resident grid, with a grid-wide
  * barrier before every step whose `sync_before` is set (= it reads what an earlier step wrote).  Every step needs its work

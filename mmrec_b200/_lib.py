@@ -30,6 +30,9 @@ PROTOTYPES = {
                               _f32, _p, _i64, _p]),
     "mmrec_spmm_acc_f32": (_i32, [_i64, _i64, _i32, _p, _p, _p, _p, _i64, _i64, _p, _p, _p, _p, _i64, _p, _i64, _p, _p, _i64,
                                   _f32, _i32, _p]),
+    "mmrec_spmm_drop_f32": (_i32, [_i64, _i64, _i32, _p, _p, _p, _p, _i64, _i64, _p, _p, _p, _p, _i64, _p, _i64, _p, _p, _i64,
+                                   _f32, _p, _f32, _p]),
+    "mmrec_edge_keep_bits": (_i32, [_i64, _p, _f32, _p, _p, _p, _p, _p]),
     "mmrec_spmm_chain_f32": (_i32, [_i32, _i32, _p, _p]),
     "mmrec_spmm_steps_f32": (_i32, [_i32, _i32, _p, _i32, _p]),
     "mmrec_project_set_path": (_i32, [_i32]),

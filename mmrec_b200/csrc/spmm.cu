@@ -132,10 +132,19 @@ __device__ __forceinline__ void spmm_epilogue(const SpmmParams& p, bool on, int 
 // travel while they are.  `maxlen` is the trip bound shared by every group that runs in lock step with this one.
 // TWO: each gathered row is read from the block of X it falls in; the products and their order are the same as from the
 // concatenation, so the result is bit-identical.
-template <int D, int T, bool TWO>
-__device__ __forceinline__ void spmm_gather(const SpmmParams& p, int b, int len, int maxlen, int l, float4 (&acc)[VecCfg<D, T>::V]) {
+// DROP: entry e (CSR position) takes part iff bit e of `dk.keep` is set, with weight fl(vals[e] * dk.scale); a dropped entry
+// is a padding slot (no load of its row of X, weight 0), so the kept entries are summed in the order of the compacted row.
+struct DropKeep { const uint32_t* keep; float scale; };
+
+__device__ __forceinline__ bool keep_bit(const uint32_t* keep, int pos) {
+    return (__ldg(keep + (pos >> 5)) >> (pos & 31)) & 1u;
+}
+
+template <int D, int T, bool TWO, bool DROP = false>
+__device__ __forceinline__ void spmm_gather(const SpmmParams& p, int b, int len, int maxlen, int l, float4 (&acc)[VecCfg<D, T>::V],
+                                            const DropKeep dk = DropKeep{nullptr, 1.f}) {
     using C = VecCfg<D, T>;
-    int cj[C::UNR]; float wj[C::UNR];
+    int cj[C::UNR]; float wj[C::UNR]; bool kj[C::UNR];
     const int32_t* cp = p.colidx + b;                                // walked with immediate offsets: no per-load address math
     const float* vp = p.vals + b;
     const float* xl = p.X + l * 4;
@@ -145,12 +154,16 @@ __device__ __forceinline__ void spmm_gather(const SpmmParams& p, int b, int len,
         const bool ok = u < len;
         cj[u] = ok ? __ldg(cp + u) : 0;
         wj[u] = ok ? __ldg(vp + u) : 0.f;
+        if constexpr (DROP) {
+            kj[u] = ok && keep_bit(dk.keep, b + u);
+            wj[u] = kj[u] ? __fmul_rn(wj[u], dk.scale) : 0.f;
+        }
     }
     for (int j0 = 0; j0 < maxlen; j0 += C::UNR, cp += C::UNR, vp += C::UNR) {
         float4 x[C::UNR][C::V];
 #pragma unroll
         for (int u = 0; u < C::UNR; ++u) {
-            const bool ok = j0 + u < len;
+            const bool ok = DROP ? kj[u] : j0 + u < len;
             const bool hi = TWO && cj[u] >= p.x_split;
             const float* xb = hi ? xh : xl;
             const uint32_t sb = hi ? p.sx_hi : p.sx;
@@ -167,6 +180,10 @@ __device__ __forceinline__ void spmm_gather(const SpmmParams& p, int b, int len,
             const bool ok = j0 + C::UNR + u < len;
             cj[u] = ok ? __ldg(cp + C::UNR + u) : 0;
             wj[u] = ok ? __ldg(vp + C::UNR + u) : 0.f;
+            if constexpr (DROP) {
+                kj[u] = ok && keep_bit(dk.keep, b + j0 + C::UNR + u);
+                wj[u] = kj[u] ? __fmul_rn(wj[u], dk.scale) : 0.f;
+            }
         }
 #pragma unroll
         for (int u = 0; u < C::UNR; ++u) {
@@ -245,8 +262,8 @@ __device__ __forceinline__ bool spmm_split_finish(const SpmmParams& p, bool spli
 // predicated, no shuffles in the gather loop (the T lanes of a group read the same (col, val) address = one
 // broadcast transaction).  Warps walk the sorted list boustrophedon, so whoever got the longest tasks in one sweep
 // gets the shortest in the next.
-template <int D, int T, bool TWO>
-__device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __restrict__ red) {
+template <int D, int T, bool TWO, bool DROP = false>
+__device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __restrict__ red, const DropKeep dk = DropKeep{nullptr, 1.f}) {
     using C = VecCfg<D, T>;
     constexpr int G = 256 / T;                              // lane groups per CTA
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -275,7 +292,7 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
         float4 acc[C::V];
 #pragma unroll
         for (int v = 0; v < C::V; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-        spmm_gather<D, T, TWO>(p, mb, mylen, chunk, l, acc);
+        spmm_gather<D, T, TWO, DROP>(p, mb, mylen, chunk, l, acc, dk);
 #pragma unroll
         for (int v = 0; v < C::V; ++v) *reinterpret_cast<float4*>(red + gi * D + (v * T + l) * 4) = acc[v];
         __syncthreads();
@@ -329,7 +346,7 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
         float4 acc[C::V];
 #pragma unroll
         for (int v = 0; v < C::V; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-        spmm_gather<D, T, TWO>(p, b, valid ? len : 0, maxlen, l, acc);
+        spmm_gather<D, T, TWO, DROP>(p, b, valid ? len : 0, maxlen, l, acc, dk);
         bool do_epi = valid && sid < 0;
         const bool split = valid && sid >= 0;
         if (__any_sync(0xffffffffu, split)) {
@@ -343,6 +360,38 @@ template <int D, int T>
 __global__ void __launch_bounds__(256) spmm_vec_kernel(const SpmmParams p) {
     __shared__ __align__(16) float red[(256 / T) * D];
     spmm_vec_body<D, T, false>(p, red);
+}
+
+// K1 with an edge-keep mask (mmrec_spmm_drop_f32): the same plan, split rows, segment-order reduction and epilogues, over
+// the entries whose keep bit is set, each weighted fl(v * scale) -- SelfCF's per-batch `sparse_dropout` of the normalised
+// adjacency (encoders.py:77-88) without rebuilding the matrix.
+template <int D, int T>
+__global__ void __launch_bounds__(256) spmm_drop_kernel(const SpmmParams p, const uint32_t* __restrict__ keep, float scale) {
+    __shared__ __align__(16) float red[(256 / T) * D];
+    spmm_vec_body<D, T, false, true>(p, red, DropKeep{keep, scale});
+}
+
+// The keep bits of one dropout draw (mmrec_edge_keep_bits): CSR position e is kept iff floor(keep_prob + draws[draw_of[e]])
+// != 0 in fp32, and its mirror bit (the transpose's position e) is the bit of position mirror[e].  One thread per position,
+// a warp per 32-bit word: the words are assembled by ballot, no atomics.
+__global__ void __launch_bounds__(256) edge_keep_bits_kernel(int64_t nnz, const float* __restrict__ draws, float keep_prob,
+                                                             const int32_t* __restrict__ draw_of, const int32_t* __restrict__ mirror,
+                                                             uint32_t* __restrict__ keep, uint32_t* __restrict__ keep_t) {
+    const int64_t n_words = (nnz + 31) >> 5;
+    const int lane = threadIdx.x & 31;
+    const int64_t w0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    auto kept = [&](int64_t e) { return floorf(__fadd_rn(keep_prob, __ldg(draws + __ldg(draw_of + e)))) != 0.f; };
+    for (int64_t w = w0; w < n_words; w += n_warps) {                // warp-uniform trip count
+        const int64_t e = (w << 5) + lane;
+        const bool in = e < nnz;
+        const uint32_t word = __ballot_sync(0xffffffffu, in && kept(e));
+        const uint32_t word_t = keep_t ? __ballot_sync(0xffffffffu, in && kept(__ldg(mirror + e))) : 0u;
+        if (lane == 0) {
+            keep[w] = word;
+            if (keep_t) keep_t[w] = word_t;
+        }
+    }
 }
 
 // Several SpMMs in one persistent launch: the steps run in order on the same grid, a CTA that is done with one step starts
@@ -401,11 +450,12 @@ __global__ void __launch_bounds__(256) spmm_generic_kernel(const SpmmParams p) {
 static thread_local int g_spmm_y_acc = 0;   // set by mmrec_spmm_acc_f32 around its call of mmrec_spmm_f32
 int g_spmm_lanes = 0;   // 0 = default lanes per task for the width; set by mmrec_spmm_set_lanes (tuning knob)
 
-template <int D, int T>
-static int launch_vec(const SpmmParams& p, cudaStream_t stream) {
+template <int D, int T, bool DROP = false>
+static int launch_vec(const SpmmParams& p, cudaStream_t stream, const DropKeep dk = DropKeep{nullptr, 1.f}) {
     static int blocks_per_sm = 0;
     if (!blocks_per_sm) {
-        MMREC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, spmm_vec_kernel<D, T>, 256, 0));
+        if constexpr (DROP) MMREC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, spmm_drop_kernel<D, T>, 256, 0));
+        else MMREC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, spmm_vec_kernel<D, T>, 256, 0));
         if (blocks_per_sm < 1) blocks_per_sm = 1;
     }
     const int64_t n_work = p.tasks ? p.n_tasks : p.n_rows;
@@ -415,7 +465,8 @@ static int launch_vec(const SpmmParams& p, cudaStream_t stream) {
     const int64_t cap = (int64_t)sm_count() * blocks_per_sm;
     if (grid > cap) grid = cap;
     if (grid < 1) return MMREC_OK;
-    spmm_vec_kernel<D, T><<<(unsigned)grid, 256, 0, stream>>>(p);
+    if constexpr (DROP) spmm_drop_kernel<D, T><<<(unsigned)grid, 256, 0, stream>>>(p, dk.keep, dk.scale);
+    else spmm_vec_kernel<D, T><<<(unsigned)grid, 256, 0, stream>>>(p);
     MMREC_LAUNCH_CHECK();
     return MMREC_OK;
 }
@@ -442,21 +493,18 @@ extern "C" int mmrec_spmm_set_lanes(int lanes_per_row) {
     return MMREC_OK;
 }
 
-extern "C" int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
-                              const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks,
-                              const int32_t* split_rows,
-                              int32_t* counters, float* partial, const float* X, int64_t ldx, float* Y, int64_t ldy,
-                              const float* acc_in, float* acc_out, int64_t ldacc, float acc_div, const float* gate_ref,
-                              int64_t ldgate, void* stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    MMREC_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && d >= 1, "spmm: bad sizes");
-    if (n_rows == 0) return MMREC_OK;
+namespace mmrec {
+// The argument checks and parameter block shared by mmrec_spmm_f32 and mmrec_spmm_drop_f32; sets *vec_ok when the operands
+// are 16-byte aligned (the vector kernel's float4 rows).
+static int spmm_params(SpmmParams& p, bool& vec_ok, int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
+                       const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks, const int32_t* split_rows,
+                       int32_t* counters, float* partial, const float* X, int64_t ldx, float* Y, int64_t ldy, const float* acc_in,
+                       float* acc_out, int64_t ldacc, float acc_div, const float* gate_ref, int64_t ldgate) {
     MMREC_CHECK_ARG(rowptr && X && (Y || acc_out), "spmm: null pointer");
     MMREC_CHECK_ARG(ldx >= d && (!Y || ldy >= d) && (!acc_out || ldacc >= d) && (!gate_ref || ldgate >= d), "spmm: leading dimension < d");
     MMREC_CHECK_ARG(acc_div != 0.0f, "spmm: acc_div == 0");
     MMREC_CHECK_ARG(!tasks || (n_tasks >= 0 && n_cta_tasks >= 0 && n_cta_tasks <= n_tasks && split_rows && counters && partial),
                     "spmm: plan pointers missing");
-    SpmmParams p;
     p.n_rows = n_rows; p.n_cols = n_cols; p.rowptr = rowptr; p.colidx = colidx; p.vals = vals;
     p.tasks = (const int4*)tasks; p.n_tasks = n_tasks; p.n_heavy = tasks ? n_cta_tasks : 0; p.split_rows = (const int4*)split_rows;
     p.counters = counters; p.partial = partial; p.X = X; p.ldx = ldx; p.Y = Y; p.ldy = ldy;
@@ -469,8 +517,25 @@ extern "C" int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d, const int32
     p.sx = (uint32_t)(ldx * 4); p.sy = (uint32_t)(ldy * 4); p.sacc = (uint32_t)(ldacc * 4); p.sgate = (uint32_t)(ldgate * 4);
     p.X_hi = X; p.x_split = (int)n_cols; p.sx_hi = p.sx; p.acc_in_hi = acc_in; p.acc_split = (int)n_rows; p.sacc_hi = p.sacc;
     auto al16 = [](const void* q, int64_t ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld & 3) == 0); };
-    const bool vec_ok = al16(X, ldx) && al16(Y, ldy) && al16(acc_in, ldacc) && al16(acc_out, ldacc) &&
-                        al16(gate_ref, ldgate) && al16(partial, 4);
+    vec_ok = al16(X, ldx) && al16(Y, ldy) && al16(acc_in, ldacc) && al16(acc_out, ldacc) && al16(gate_ref, ldgate) && al16(partial, 4);
+    return MMREC_OK;
+}
+}  // namespace mmrec
+
+extern "C" int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
+                              const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks,
+                              const int32_t* split_rows,
+                              int32_t* counters, float* partial, const float* X, int64_t ldx, float* Y, int64_t ldy,
+                              const float* acc_in, float* acc_out, int64_t ldacc, float acc_div, const float* gate_ref,
+                              int64_t ldgate, void* stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    MMREC_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && d >= 1, "spmm: bad sizes");
+    if (n_rows == 0) return MMREC_OK;
+    SpmmParams p;
+    bool vec_ok = false;
+    const int rc = spmm_params(p, vec_ok, n_rows, n_cols, d, rowptr, colidx, vals, tasks, n_tasks, n_cta_tasks, split_rows, counters,
+                               partial, X, ldx, Y, ldy, acc_in, acc_out, ldacc, acc_div, gate_ref, ldgate);
+    if (rc != MMREC_OK) return rc;
     if (vec_ok) {
         switch (d) {
             case 32: return launch_vec_d<32>(p, stream);
@@ -485,6 +550,48 @@ extern "C" int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d, const int32
     const int64_t cap = (int64_t)sm_count() * 8;
     if (grid > cap) grid = cap;
     spmm_generic_kernel<<<(unsigned)grid, 256, 0, stream>>>(p);
+    MMREC_LAUNCH_CHECK();
+    return MMREC_OK;
+}
+
+extern "C" int mmrec_spmm_drop_f32(int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
+                                   const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks,
+                                   const int32_t* split_rows, int32_t* counters, float* partial, const float* X, int64_t ldx,
+                                   float* Y, int64_t ldy, const float* acc_in, float* acc_out, int64_t ldacc, float acc_div,
+                                   const uint32_t* keep_bits, float scale, void* stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    MMREC_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && d >= 1, "spmm_drop: bad sizes");
+    if (n_rows == 0) return MMREC_OK;
+    MMREC_CHECK_ARG(keep_bits, "spmm_drop: keep_bits is null");
+    SpmmParams p;
+    bool vec_ok = false;
+    const int rc = spmm_params(p, vec_ok, n_rows, n_cols, d, rowptr, colidx, vals, tasks, n_tasks, n_cta_tasks, split_rows, counters,
+                               partial, X, ldx, Y, ldy, acc_in, acc_out, ldacc, acc_div, nullptr, 0);
+    if (rc != MMREC_OK) return rc;
+    if (!vec_ok || !(d == 32 || d == 64 || d == 128 || d == 256)) {
+        set_error("spmm_drop: d = %d or unaligned operands: the masked kernel is built for 16-byte aligned d in {32, 64, 128, 256}", d);
+        return MMREC_EUNSUPPORTED;
+    }
+    const DropKeep dk{keep_bits, scale};
+    switch (d) {                                      // one float4 per lane, the default of the unmasked kernel
+        case 32: return launch_vec<32, 8, true>(p, stream, dk);
+        case 64: return launch_vec<64, 16, true>(p, stream, dk);
+        case 128: return launch_vec<128, 32, true>(p, stream, dk);
+        default: return launch_vec<256, 32, true>(p, stream, dk);
+    }
+}
+
+extern "C" int mmrec_edge_keep_bits(int64_t nnz, const float* draws, float keep_prob, const int32_t* draw_of, const int32_t* mirror,
+                                    uint32_t* keep_bits, uint32_t* keep_bits_t, void* stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    MMREC_CHECK_ARG(nnz >= 0 && nnz < (1ll << 31), "edge_keep_bits: nnz out of range");
+    if (nnz == 0) return MMREC_OK;
+    MMREC_CHECK_ARG(draws && draw_of && keep_bits && (!keep_bits_t || mirror), "edge_keep_bits: null pointer");
+    const int64_t n_words = (nnz + 31) / 32;
+    int64_t grid = (n_words + 7) / 8;                 // 8 warps per block, one word per warp
+    const int64_t cap = (int64_t)sm_count() * 16;
+    if (grid > cap) grid = cap;
+    edge_keep_bits_kernel<<<(unsigned)grid, 256, 0, stream>>>(nnz, draws, keep_prob, draw_of, mirror, keep_bits, keep_bits_t);
     MMREC_LAUNCH_CHECK();
     return MMREC_OK;
 }

@@ -62,6 +62,39 @@ def mgcn_norm_adj_entries(inter_row, inter_col, n_users, n_items):
     return rows, cols, vals
 
 
+def dropout_entry_maps(inter_row, inter_col, n_users, n_items):
+    """The two index maps of SelfCF's per-batch edge dropout on `build_norm_adj`'s CSR (`src/common/encoders.py:77-88`):
+
+    * `draw_of` int32[nnz]: draw j of `torch.rand(nnz)` belongs to the reference's j-th stored entry of `sparse_norm_adj`,
+      which is CSR position e with draw_of[e] = j;
+    * `mirror` int32[nnz]: the CSR position of (c, r) for the entry (r, c) at position e (the matrix is symmetric, so the
+      dropped matrix's transpose is the same CSR with the keep bits read through `mirror`).
+
+    The reference's stored order is that of `sp.coo_matrix(D * A * D)` with `A` the dok built from a dict
+    (`encoders.py:51-70`).  With the scipy of this image (1.18) that order is: rows ascending, and within a row the
+    first-insertion order of the dict -- the interaction COO's (u, i + n_users) pairs, then its (i + n_users, u) pairs, a
+    repeated pair at its first position.  (Measured; it is the order of `A.tocsr()`.  Another scipy may store the product
+    differently: the masks then match in distribution only.)  So the order is a stable sort by row of the de-duplicated
+    concatenation, and each of its keys is found in the sorted keys of the CSR; no dok or scipy product is built."""
+    r = np.asarray(inter_row, dtype=np.int64)
+    c = np.asarray(inter_col, dtype=np.int64)
+    n = n_users + n_items
+    key = np.concatenate([r * n + (c + n_users), (c + n_users) * n + r])
+    order = np.argsort(key, kind="stable")                           # equal keys keep their order: the first occurrence leads
+    s = key[order]
+    start = np.empty(s.size, dtype=bool)
+    if s.size:
+        start[0] = True
+        np.not_equal(s[1:], s[:-1], out=start[1:])
+    ukey = s[start]                                                   # = the CSR's (row, col) keys in CSR order
+    first = order[start]                                              # first position of each key in the concatenation
+    ref = np.lexsort((first, ukey // n))                             # CSR positions in the reference's stored order
+    draw_of = np.empty(ukey.size, dtype=np.int32)
+    draw_of[ref] = np.arange(ukey.size, dtype=np.int32)
+    mirror = np.searchsorted(ukey, (ukey % n) * n + ukey // n).astype(np.int32)
+    return draw_of, mirror
+
+
 def _to_dev(a, device, dtype=None):
     t = torch.from_numpy(np.ascontiguousarray(a))
     return t.to(device=device, dtype=dtype) if dtype is not None else t.to(device)

@@ -207,9 +207,13 @@ class PanelCSR:
 
 def spmm_raw(A, X: torch.Tensor, Y: Optional[torch.Tensor] = None, acc_in: Optional[torch.Tensor] = None,
              acc_out: Optional[torch.Tensor] = None, acc_div: float = 1.0, gate_ref: Optional[torch.Tensor] = None,
-             use_plan: bool = True, y_accumulate: bool = False):
+             use_plan: bool = True, y_accumulate: bool = False, drop: Optional[tuple] = None):
     """y = A X with the fused epilogue of include/mmrec_b200.h (no autograd).  Replaces `torch.sparse.mm`
-    (`src/models/freedom.py:167,172`) plus the stack/mean (`:175-176`) and `+ h` (`:178`) that follow."""
+    (`src/models/freedom.py:167,172`) plus the stack/mean (`:175-176`) and `+ h` (`:178`) that follow.
+    `drop` = (keep_bits, scale): only the entries whose keep bit is set take part, weighted fl(v * scale)
+    (`mmrec_spmm_drop_f32`; SelfCF's `sparse_dropout`, `src/common/encoders.py:77-88`)."""
+    if drop is not None and (isinstance(A, PanelCSR) or gate_ref is not None or y_accumulate):
+        raise MMRecError("spmm: the edge-keep mask runs on a CSR without the gate or y_accumulate")
     if isinstance(A, PanelCSR):
         if gate_ref is not None:
             raise MMRecError("spmm: the cosine gate needs the whole row sum: not available on a PanelCSR")
@@ -240,6 +244,18 @@ def spmm_raw(A, X: torch.Tensor, Y: Optional[torch.Tensor] = None, acc_in: Optio
                                      _ptr(A.partial(d)) if plan else None,
                                      _ptr(X), X.stride(0), _ptr(Y), d, _ptr(acc_in), _ptr(acc_out), d, float(acc_div), 1, _stream()),
               "mmrec_spmm_acc_f32")
+        return
+    if drop is not None:
+        keep, scale = drop
+        _need_cuda(keep)
+        if keep.dtype != torch.int32 or not keep.is_contiguous() or keep.numel() < (A.nnz + 31) // 32:
+            raise MMRecError("spmm: keep_bits must be contiguous int32 [ceil(nnz / 32)]")
+        check(lib.mmrec_spmm_drop_f32(A.n_rows, A.n_cols, d, _ptr(A.rowptr), _ptr(A.colidx), _ptr(A.vals),
+                                      _ptr(A.tasks) if plan else None, A.n_tasks if plan else 0, A.n_cta_tasks if plan else 0,
+                                      _ptr(A.split_rows) if plan else None, _ptr(A.counters) if plan else None,
+                                      _ptr(A.partial(d)) if plan else None,
+                                      _ptr(X), X.stride(0), _ptr(Y), d, _ptr(acc_in), _ptr(acc_out), d, float(acc_div),
+                                      _ptr(keep), float(scale), _stream()), "mmrec_spmm_drop_f32")
         return
     check(lib.mmrec_spmm_f32(A.n_rows, A.n_cols, d, _ptr(A.rowptr), _ptr(A.colidx), _ptr(A.vals),
                              _ptr(A.tasks) if plan else None, A.n_tasks if plan else 0, A.n_cta_tasks if plan else 0,
@@ -374,17 +390,20 @@ def _propagate_mean_post_unfused(A, ego, n_layers, post_csr, post_x, post_layers
 
 class _PropagateMeanFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, ego, A: CSR, n_layers: int):
-        ctx.A, ctx.L = A, n_layers
+    def forward(ctx, ego, A: CSR, n_layers: int, drop: Optional[tuple] = None):
+        # drop = (keep_bits, keep_bits_t, scale) of a symmetric A: the forward multiplies by the dropped matrix, the backward
+        # by its transpose, which is the same CSR with the mirrored bits
+        ctx.A, ctx.L, ctx.drop = A, n_layers, drop
         ego = _f32c(ego)
         if n_layers == 0:
             return ego.clone()
+        fwd = None if drop is None else (drop[0], drop[2])
         acc = torch.empty_like(ego)
         x = ego
         for l in range(1, n_layers + 1):
             last = l == n_layers
             y = None if last else torch.empty_like(ego)
-            spmm_raw(A, x, Y=y, acc_in=ego if l == 1 else acc, acc_out=acc, acc_div=float(n_layers + 1) if last else 1.0)
+            spmm_raw(A, x, Y=y, acc_in=ego if l == 1 else acc, acc_out=acc, acc_div=float(n_layers + 1) if last else 1.0, drop=fwd)
             x = y
         return acc
 
@@ -393,14 +412,16 @@ class _PropagateMeanFn(torch.autograd.Function):
         L = ctx.L
         gm = _f32c(g) / float(L + 1)                # d mean / d E_l, the same for every layer
         if L == 0:
-            return g, None, None
-        At = ctx.A.t()
+            return g, None, None, None
+        drop = ctx.drop
+        At = ctx.A.t() if drop is None else ctx.A
+        bwd = None if drop is None else (drop[1], drop[2])
         cur = gm
         for _ in range(L):                          # g_l = gm + A^T g_{l+1}
             nxt = torch.empty_like(gm)
-            spmm_raw(At, cur, acc_in=gm, acc_out=nxt)
+            spmm_raw(At, cur, acc_in=gm, acc_out=nxt, drop=bwd)
             cur = nxt
-        return cur, None, None
+        return cur, None, None, None
 
 
 def propagate_mean(A: CSR, ego: torch.Tensor, n_layers: int) -> torch.Tensor:
@@ -408,6 +429,40 @@ def propagate_mean(A: CSR, ego: torch.Tensor, n_layers: int) -> torch.Tensor:
     (`src/models/freedom.py:169-176`, `bm3.py:86-92`, `lightgcn.py:116-123`, `mgcn.py:159-166`), with the
     running sum and the final division fused into the SpMM epilogue (no stack, no extra passes)."""
     return _PropagateMeanFn.apply(ego, A, n_layers)
+
+
+def edge_keep_bits(draws: torch.Tensor, keep_prob: float, draw_of: torch.Tensor, mirror: Optional[torch.Tensor] = None):
+    """The keep bits of one `sparse_dropout` draw (`src/common/encoders.py:77-84`): `floor(float32(1 - rate) + draws)`
+    with one fp32 add, draw j applied to the CSR position e with draw_of[e] = j (`graph.dropout_entry_maps`).  Returns
+    (keep_bits, keep_bits_t) as int32 [ceil(nnz / 32)] (bit e of word e // 32); keep_bits_t (None without `mirror`) holds
+    bit mirror[e] of keep_bits at e: the transpose of the dropped symmetric matrix on the same CSR."""
+    _need_cuda(draws, draw_of, mirror)
+    draws = _f32c(draws)
+    nnz = draws.numel()
+    for name, t in (("draw_of", draw_of), ("mirror", mirror)):
+        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != nnz):
+            raise MMRecError(f"edge_keep_bits: {name} must be contiguous int32 [{nnz}]")
+    n_words = (nnz + 31) // 32
+    if n_words == 0:                                # nothing to launch: one word of zeros, as "bits past nnz are 0" promises
+        keep = torch.zeros(1, dtype=torch.int32, device=draws.device)
+        return keep, None if mirror is None else torch.zeros_like(keep)
+    keep = torch.empty(n_words, dtype=torch.int32, device=draws.device)
+    keep_t = None if mirror is None else torch.empty_like(keep)
+    check(_lib.load().mmrec_edge_keep_bits(nnz, _ptr(draws), float(keep_prob), _ptr(draw_of), _ptr(mirror), _ptr(keep), _ptr(keep_t),
+                                           _stream()), "mmrec_edge_keep_bits")
+    return keep, keep_t
+
+
+def propagate_mean_dropped(A: CSR, ego: torch.Tensor, n_layers: int, keep: torch.Tensor, keep_t: torch.Tensor,
+                           scale: float) -> torch.Tensor:
+    """`propagate_mean` through the edge-dropped matrix of SelfCF's encoder (`src/common/encoders.py:90-112`: `sparse_dropout`
+    of the normalised adjacency, then `torch.sparse.mm` per layer and the layer mean), on the fixed CSR and its fixed plan:
+    the entries whose bit of `keep` is set, weighted fl(v * scale) (`mmrec_spmm_drop_f32`).  Differentiable w.r.t. `ego`; the
+    backward runs the same CSR with `keep_t` (`edge_keep_bits` with the mirror map), as A is symmetric bit for bit."""
+    if not A.symmetric:
+        raise MMRecError("propagate_mean_dropped: the backward reads the transpose through the mirrored bits; A must be symmetric")
+    _need_cuda(ego, keep, keep_t)
+    return _PropagateMeanFn.apply(ego, A, n_layers, (keep, keep_t, float(scale)))
 
 
 def propagate_layergcn(A: CSR, ego: torch.Tensor, n_layers: int) -> torch.Tensor:
