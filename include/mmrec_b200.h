@@ -95,12 +95,16 @@ int mmrec_bipartite_norm_f32(int64_t n_edges, const int64_t* users, const int64_
  *   if acc_out:  acc_out[r,:] = ((acc_in ? acc_in[r,:] : 0) + y[r,:]) / acc_div
  *
  * acc_in may alias acc_out.  d in {32, 64, 128, 256} runs the vectorised kernel, any other d >= 1
- * the generic one.  tasks/n_tasks/n_cta_tasks/split_rows/counters/partial come from mmrec_spmm_plan
+ * the generic one.  d in {96, 192, 384} = 3 x {32, 64, 128} (several d-wide operands side by side,
+ * SLMRec's three views) also runs the vectorised kernel, three float4 per lane on the lanes the width
+ * d/3 uses: without the gate, every d/3-wide column block of the result is bit-identical to the
+ * width-d/3 product of that block.  The lane override does not apply to these widths.  tasks/n_tasks/n_cta_tasks/split_rows/counters/partial come from mmrec_spmm_plan
  * (counters: int32[n_split_rows], zero on entry and zero again on exit; partial:
  * fp32[n_slots * d]); tasks == NULL selects one warp per row.  Summation order is fixed, so the
  * result is bit-reproducible run to run.
  * ------------------------------------------------------------------------------------------- */
-/* tuning knob: lanes that cooperate on one row (0 = default min(32, d/4); a power of two, d/(4*lanes) float4 per lane) */
+/* tuning knob: lanes that cooperate on one row (0 = default min(32, d/4); a power of two, d/(4*lanes) float4 per lane;
+ * d in {32, 64, 128, 256} only) */
 int mmrec_spmm_set_lanes(int lanes_per_row);
 int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d,
                    const int32_t* rowptr, const int32_t* colidx, const float* vals,

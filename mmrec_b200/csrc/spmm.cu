@@ -67,7 +67,10 @@ struct VecCfg {
     static_assert(D % (4 * T) == 0, "row must split into float4 per lane");
     static constexpr int V = D / (4 * T);              // float4 per lane per row of X
     static constexpr int GPW = 32 / T;                 // tasks per warp
-    static constexpr int UNR = (V >= 4) ? 2 : (V == 2 ? 4 : 8);   // rows of X in flight per lane group
+    // rows of X in flight per lane group.  V = 3 (the width-3d instances): 4 rows, 12 float4 per lane -- 86 registers, no
+    // spills, 2 CTAs of 256 threads per SM; 8 would be 24 float4 and ~102 registers, 2 would be 80 registers and 3 CTAs but
+    // fewer rows in flight per SM (DESIGN.md section 4, K1)
+    static constexpr int UNR = (V >= 4) ? 2 : (V == 3 ? 4 : (V == 2 ? 4 : 8));
 };
 
 template <int D, int T>
@@ -482,6 +485,17 @@ static int launch_vec_d(const SpmmParams& p, cudaStream_t stream) {
     return launch_vec<D, T8>(p, stream);
 }
 
+// The widths 3d (d = 32, 64, 128): three float4 per lane, T = D / 12 -- the lane count of the width-d default (one float4
+// per lane at d = D / 3).  Lane l owns float4 v * T + l of a row, so float4 block v is column block v, and every lane group,
+// CTA reduction, split-row partial and epilogue sums block v exactly as the width-d kernel sums its row: each column block
+// of the width-3d product is the width-d product of that block, bit for bit (not under the cosine gate, which reduces over
+// the whole row).  The lane override does not apply to these widths.
+template <int D>
+static int launch_vec_3d(const SpmmParams& p, cudaStream_t stream) {
+    static_assert(VecCfg<D, D / 12>::V == 3, "three float4 per lane");
+    return launch_vec<D, D / 12>(p, stream);
+}
+
 }  // namespace mmrec
 
 using namespace mmrec;
@@ -542,6 +556,9 @@ extern "C" int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d, const int32
             case 64: return launch_vec_d<64>(p, stream);
             case 128: return launch_vec_d<128>(p, stream);
             case 256: return launch_vec_d<256>(p, stream);
+            case 96: return launch_vec_3d<96>(p, stream);
+            case 192: return launch_vec_3d<192>(p, stream);
+            case 384: return launch_vec_3d<384>(p, stream);
             default: break;
         }
     }

@@ -62,6 +62,58 @@ def mgcn_norm_adj_entries(inter_row, inter_col, n_users, n_items):
     return rows, cols, vals
 
 
+SLMREC_SYMMETRIC_ADJ = ("plain", "pre")
+
+
+def slmrec_adj_entries(inter_row, inter_col, n_users, n_items, adj_type):
+    """(rows, cols, vals fp32) of SLMRec's `create_adj_mat` (`src/models/slmrec.py:434-479`) for each `adj_type`, with the
+    dtypes its scipy calls compute in, so that the values equal the fp32 ones it hands to `torch.sparse.FloatTensor`:
+
+    * `plain`: the binary symmetric A (float32 ones);
+    * `norm`: D^-1 (A + I) -- `sp.eye` is float64, so the degrees + 1 and `np.power(., -1)` are float64, rounded to fp32 once;
+    * `gcmc`: D^-1 A in float32 (`np.power(deg, -1)` of the float32 degrees, inf -> 0);
+    * `pre`: D^-1/2 A D^-1/2 in float32: `deg + 1e-08` and `np.power(., -0.5)` in float32, one fp32 product per entry;
+    * anything else (`mean`): the float32 D^-1 A of `gcmc` plus I, the diagonal 1.0.
+
+    Only `plain` and `pre` are symmetric (SLMREC_SYMMETRIC_ADJ).  Entries in (row, col) order."""
+    rows, cols, n = _sym_keys(inter_row, inter_col, n_users, n_items)
+    deg = np.bincount(rows, minlength=n)
+    if adj_type == "plain":
+        return rows, cols, np.ones(rows.size, dtype=np.float32)
+    if adj_type == "pre":
+        with np.errstate(divide="ignore"):
+            dinv = np.power(deg.astype(np.float32) + 1e-08, -0.5)
+        dinv[np.isinf(dinv)] = 0.0
+        return rows, cols, (dinv[rows] * dinv[cols]).astype(np.float32)
+    if adj_type == "norm":
+        dinv = np.power(deg.astype(np.float64) + 1.0, -1)
+        diag = np.arange(n, dtype=np.int64)
+        key = np.concatenate([rows * n + cols, diag * n + diag])
+        order = np.argsort(key, kind="stable")
+        r, c = key[order] // n, key[order] % n
+        return r, c, dinv[r].astype(np.float32)
+    with np.errstate(divide="ignore"):
+        dinv = np.power(deg.astype(np.float32), -1)
+    dinv[np.isinf(dinv)] = 0.0
+    if adj_type == "gcmc":
+        return rows, cols, dinv[rows].astype(np.float32)
+    diag = np.arange(n, dtype=np.int64)                               # mean: D^-1 A + I (bipartite: no diagonal in D^-1 A)
+    key = np.concatenate([rows * n + cols, diag * n + diag])
+    vals = np.concatenate([dinv[rows].astype(np.float32), np.ones(n, dtype=np.float32)])
+    order = np.argsort(key, kind="stable")
+    return key[order] // n, key[order] % n, vals[order]
+
+
+def build_slmrec_adj(inter, n_users, n_items, device, adj_type) -> CSR:
+    """SLMRec's `norm_adj` (`slmrec.py:40-44`) as a device CSR; flagged symmetric for `plain` and `pre` only, so the
+    others take their backward on `CSR.t()`."""
+    r, c = (inter.row, inter.col) if hasattr(inter, "row") else inter
+    rows, cols, vals = slmrec_adj_entries(r, c, n_users, n_items, adj_type)
+    n = n_users + n_items
+    return CSR.from_coo(_to_dev(rows, device), _to_dev(cols, device), _to_dev(vals, device), n, n,
+                        sum_duplicates=False, symmetric=adj_type in SLMREC_SYMMETRIC_ADJ)
+
+
 def dropout_entry_maps(inter_row, inter_col, n_users, n_items):
     """The two index maps of SelfCF's per-batch edge dropout on `build_norm_adj`'s CSR (`src/common/encoders.py:77-88`):
 
