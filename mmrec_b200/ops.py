@@ -47,6 +47,13 @@ def _f32c(t: torch.Tensor) -> torch.Tensor:
     return t if t.is_contiguous() else t.contiguous()
 
 
+def _refuse_capture(op: str):
+    """Raise before anything is enqueued when the current stream is capturing a CUDA graph: `op` reads a count back to the
+    host (a synchronising copy), which would invalidate the capture, or bake the count seen at capture time into the graph."""
+    if torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing():     # (no capture before CUDA is set up)
+        raise MMRecError(f"{op} reads a result back to the host and cannot be captured in a CUDA graph: run it eagerly")
+
+
 def _ws(name: str, nbytes: int, device) -> torch.Tensor:
     """Scratch for one op family, per device AND per stream (two streams never share a buffer).  A buffer that turned
     out too small is kept alive next to its replacement: a CUDA graph captured earlier has its address baked in."""
@@ -76,13 +83,14 @@ class CSR:
         self.seg = SEG if seg is None else seg
         self.light_max = LIGHT_MAX if light_max is None else light_max
         self._t: Optional["CSR"] = None
-        self._partial = {}
+        self._split = {}                                # (device, stream) -> split-row counters and partials, see _split_scratch
         self._plan()
 
     # -- construction ------------------------------------------------------------------------------
     @staticmethod
     def from_coo(row: torch.Tensor, col: torch.Tensor, val: Optional[torch.Tensor], n_rows: int, n_cols: int,
                  sum_duplicates: bool = True, symmetric: bool = False, seg=None, light_max=None) -> "CSR":
+        _refuse_capture("CSR.from_coo")
         _lib.require_device()
         _need_cuda(row, col, val)
         lib = _lib.load()
@@ -109,6 +117,7 @@ class CSR:
         return CSR.from_coo(idx[0], idx[1], val.to(torch.float32), t.shape[0], t.shape[1], True, symmetric)
 
     def _plan(self):
+        _refuse_capture("CSR._plan")
         lib = _lib.load()
         dev = self.rowptr.device
         max_tasks = self.n_rows + self.nnz // self.seg + 1
@@ -124,13 +133,36 @@ class CSR:
         self.n_cta_tasks = int(c[4])
         self.tasks = tasks[:4 * max(self.n_tasks, 1)]
         self.split_rows = split[:4 * max(self.n_split, 1)]
-        self.counters = torch.zeros(max(self.n_split, 1), dtype=torch.int32, device=dev)
+
+    def _split_scratch(self):
+        """The split rows' arrival counters and segment partials of the current stream, per device AND per stream like `_ws`:
+        two products of this matrix in flight on two streams must not count each other's segments or add each other's
+        partials.  The counters are zero at rest (the last segment of a row resets its counter).  Buffers are never dropped,
+        so a CUDA graph that captured their addresses stays valid.  Counters first allocated while the stream is capturing
+        are zeroed by a memset inside that graph; they are zeroed again (in the graph being captured, or eagerly) until an
+        eager call has done it."""
+        dev = self.rowptr.device
+        key = (dev.index, torch.cuda.current_stream(dev).cuda_stream)
+        s = self._split.get(key)
+        if s is None:
+            s = self._split[key] = {"counters": torch.zeros(max(self.n_split, 1), dtype=torch.int32, device=dev), "partial": {},
+                                    "zeroed": not torch.cuda.is_current_stream_capturing()}
+        elif not s["zeroed"]:
+            s["counters"].zero_()
+            s["zeroed"] = not torch.cuda.is_current_stream_capturing()
+        return s
+
+    @property
+    def counters(self) -> torch.Tensor:
+        """The split-row arrival counters of the current stream (all zero between products)."""
+        return self._split_scratch()["counters"]
 
     def partial(self, d: int) -> torch.Tensor:
-        t = self._partial.get(d)
+        """The segment partials of the current stream for width d."""
+        parts = self._split_scratch()["partial"]
+        t = parts.get(d)
         if t is None:
-            t = torch.empty(max(self.n_slots, 1) * d, dtype=torch.float32, device=self.rowptr.device)
-            self._partial[d] = t
+            t = parts[d] = torch.empty(max(self.n_slots, 1) * d, dtype=torch.float32, device=self.rowptr.device)
         return t
 
     # -- views ---------------------------------------------------------------------------------------
@@ -814,6 +846,7 @@ _last_fused: dict = {}
 def fused_fallback_rows(*_ignored) -> int:
     """Diagnostic (synchronises): how many rows of the last row block of the last fused score_topk call went through the
     exact fp32 kernel; -1 when that call did not take the fused path."""
+    _refuse_capture("fused_fallback_rows")
     if not _last_fused:
         return -1
     return int(_lib.load().mmrec_debug_fused_fallback_rows(_ptr(_last_fused["ws"]), *_last_fused["args"]))
@@ -837,7 +870,10 @@ def knn_topk(x: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None, norms
 
     With `shrink` (`mmrec_knn_topk_shrink_f32`): ranked by `(x[q] . x[i]) / (norms[q] * norms[i] + shrink)`, ItemKNNCBF's
     `build_item_sim_matrix` (`src/models/itemknncbf.py:56-65`); `norms` defaults to `torch.norm(x, p=2, dim=-1)`, the
-    reference's expression.  Bit-identical to the score, that elementwise denominator, then `mask_topk(.., None, k)`."""
+    reference's expression.  Bit-identical to the score, that elementwise denominator, then `mask_topk(.., None, k)`.
+
+    Synchronises (it reads back how many rows take the exact route): refused while the stream captures a CUDA graph."""
+    _refuse_capture("knn_topk")
     _need_cuda(x, rows, norms)
     lib = _lib.load()
     if x.dim() != 2:
@@ -876,6 +912,7 @@ def knn_topk(x: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None, norms
 def knn_fallback_rows() -> int:
     """Diagnostic: rows of the last `knn_topk` call that took the exact route (all of them when the table held a
     non-finite element); -1 before the first call."""
+    _refuse_capture("knn_fallback_rows")
     return int(_lib.load().mmrec_debug_knn_fallback_rows())
 
 
@@ -906,7 +943,10 @@ def sparse_scores(R: CSR, S: CSR, users: Optional[torch.Tensor] = None) -> torch
 def sparse_score_topk(R: CSR, S: CSR, users: Optional[torch.Tensor], mask: Optional[torch.Tensor], k: int):
     """Fused `sparse_scores` + `scores[mask[0], mask[1]] = -1e10` + top-k (`src/common/trainer.py:304-309`) without a
     dense row (`mmrec_sparse_score_topk_f32`, K9).  Returns (values [B, k], indices int64 [B, k]), bit-identical to
-    `mask_topk(sparse_scores(R, S, users), mask, k)`."""
+    `mask_topk(sparse_scores(R, S, users), mask, k)`.
+
+    Synchronises (it reads back how many rows take the unfused route): refused while the stream captures a CUDA graph."""
+    _refuse_capture("sparse_score_topk")
     users, parts = _sparse_pair(R, S, users)
     _need_cuda(mask)
     lib = _lib.load()
@@ -931,6 +971,7 @@ def sparse_score_topk(R: CSR, S: CSR, users: Optional[torch.Tensor], mask: Optio
 def sparse_topk_fallback_rows() -> int:
     """Diagnostic: rows of the last `sparse_score_topk` call served by the unfused route (too many products or masked
     items for shared memory, or a non-finite score); -1 before the first call."""
+    _refuse_capture("sparse_topk_fallback_rows")
     return int(_lib.load().mmrec_debug_sparse_topk_fallback_rows())
 
 
