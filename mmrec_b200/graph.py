@@ -163,6 +163,89 @@ def build_norm_adj(inter, n_users, n_items, device, variant="lightgcn") -> CSR:
                         sum_duplicates=False, symmetric=True)
 
 
+def gcn_add_entries(edge_index: torch.Tensor, n_nodes: int):
+    """(dst, src, norm fp32) of DualGNN's `Base_gcn` with `aggr='add'` (`src/models/dualgnn.py:325-341`), PyG's `gcn`-style
+    norm: `remove_self_loops`, `deg = degree(row)` (an fp32 `index_add` of ones), `deg.pow(-0.5)`, `norm = dis[row] *
+    dis[col]`, and the message `norm * x[row]` summed at `col`.  The same fp32 torch expressions on the host, so the values
+    equal the reference's bit for bit.  No epsilon: unlike `norm_adj_entries` a node of degree 0 has no entries to scale."""
+    ei = edge_index.detach().to("cpu", torch.int64)
+    ei = ei[:, ei[0] != ei[1]]
+    row, col = ei[0], ei[1]
+    deg = torch.zeros(n_nodes, dtype=torch.float32).index_add_(0, row, torch.ones(row.numel(), dtype=torch.float32))
+    dis = deg.pow(-0.5)
+    return col, row, dis[row] * dis[col]
+
+
+def build_gcn_add_adj(edge_index: torch.Tensor, n_nodes: int, device) -> CSR:
+    """`gcn_add_entries` as a device CSR.  Repeated edges stay separate terms, as in the reference's scatter.  The edge list
+    must hold both directions of every edge (DualGNN's, `dualgnn.py:59-60`): the matrix is then symmetric bit for bit
+    (dis[r] * dis[c] == dis[c] * dis[r]) and its backward reads the same CSR."""
+    dst, src, val = gcn_add_entries(edge_index, n_nodes)
+    return CSR.from_coo(dst.to(device), src.to(device), val.to(device), n_nodes, n_nodes, sum_duplicates=False, symmetric=True)
+
+
+class UserGraphTable:
+    """DualGNN's `user_graph_dict` (`{user: [neighbours, co-occurrence counts]}`, at most 200 per user, best first; written
+    by `preprocessing/dualgnn-gen-u-u-matrix.py` or `synth.write_user_graph_dict`) as arrays, converted once: the first
+    min(n_u, k) neighbours `idx` int64 [U, k] and their counts `w` fp32 [U, k] (zero-padded), and `n` = min(n_u, k)."""
+
+    def __init__(self, user_graph_dict: dict, k: int):
+        n_users = len(user_graph_dict)
+        self.k = k
+        self.idx = np.zeros((n_users, k), dtype=np.int64)
+        self.w = np.zeros((n_users, k), dtype=np.float32)
+        self.n = np.zeros(n_users, dtype=np.int64)
+        for u in range(n_users):                                      # the dict's keys are 0 .. U-1, as the script writes them
+            nb, wt = user_graph_dict[u][0][:k], user_graph_dict[u][1][:k]
+            m = len(nb)
+            self.n[u] = m
+            if m:
+                self.idx[u, :m] = nb
+                self.w[u, :m] = np.asarray(wt, dtype=np.float64).astype(np.float32)   # torch.tensor(list of floats): fp32
+
+    def sample(self, rng=np.random):
+        """`DualGNN.topk_sample(k)` (`dualgnn.py:207-250`) with `user_aggr_mode = 'softmax'`: (index int64 [U, k], weights fp32
+        [U, k]).  A user with 0 < n_u < k neighbours is padded by `sample.append(sample[randint(0, len(sample))])`, the bound
+        growing with each append; the draws come from `rng` (the reference's global `np.random`) in the reference's order,
+        users ascending and appends in turn, as one `randint` call with an array of bounds: the same stream as the
+        reference's scalar calls (tests/test_dualgnn_host.py).  Rows are then softmax-ed as one [U', k] fp32 tensor, the
+        same bits as the reference's per-row `F.softmax(torch.tensor(weights), dim=0)` (also tested).  A user with no
+        neighbours keeps the reference's row of index 0 with weight 0."""
+        k = self.k
+        idx, w = self.idx.copy(), self.w.copy()
+        pos = np.arange(k)
+        short = (self.n > 0) & (self.n < k)
+        pad = short[:, None] & (pos[None, :] >= self.n[:, None])    # the appended slots, row-major = the reference's draw order
+        users, slots = np.nonzero(pad)
+        if users.size:
+            draws_2d = np.zeros_like(idx)
+            draws_2d[users, slots] = rng.randint(0, slots)            # bound = len(sample) at the append = the slot
+            for p in range(int(self.n[short].min()), k):              # slot p copies an earlier slot, possibly itself a copy
+                rows = users[slots == p]
+                src = draws_2d[rows, p]
+                idx[rows, p] = idx[rows, src]
+                w[rows, p] = w[rows, src]
+        weights = np.zeros((idx.shape[0], k), dtype=np.float32)
+        have = self.n > 0
+        if have.any():
+            weights[have] = torch.softmax(torch.from_numpy(w[have]), dim=1).numpy()
+        return idx, weights
+
+
+def build_user_graph(idx: np.ndarray, weights: np.ndarray, device) -> CSR:
+    """The per-epoch user graph G [U, U]: G[u, idx[u, j]] += weights[u, j], so that `G @ X` is `User_Graph_sample`'s
+    `matmul(weights.unsqueeze(1), X[idx]).squeeze()` (`dualgnn.py:259-266`) without the [U, k, d] gather.  Repeated
+    neighbours (the padding) stay separate terms (`sum_duplicates=False`), as in the reference's product.  Users without
+    neighbours (weights 0) get no entries.  The transpose, which the backward reads, is built here too."""
+    n_users, k = idx.shape
+    keep = np.repeat(weights.any(axis=1), k)
+    rows = np.repeat(np.arange(n_users, dtype=np.int64), k)[keep]
+    G = CSR.from_coo(_to_dev(rows, device), _to_dev(idx.reshape(-1)[keep], device), _to_dev(weights.reshape(-1)[keep], device),
+                     n_users, n_users, sum_duplicates=False, symmetric=False)
+    G.t()
+    return G
+
+
 def build_mgcn_R(inter, n_users, n_items, device) -> CSR:
     """`self.R` = the U x I block of MGCN's normalised matrix (`mgcn.py:134`)."""
     r, c = (inter.row, inter.col) if hasattr(inter, "row") else inter

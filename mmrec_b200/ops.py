@@ -422,10 +422,12 @@ def _propagate_mean_post_unfused(A, ego, n_layers, post_csr, post_x, post_layers
 
 class _PropagateMeanFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, ego, A: CSR, n_layers: int, drop: Optional[tuple] = None):
+    def forward(ctx, ego, A: CSR, n_layers: int, drop: Optional[tuple] = None, div: Optional[float] = None):
         # drop = (keep_bits, keep_bits_t, scale) of a symmetric A: the forward multiplies by the dropped matrix, the backward
-        # by its transpose, which is the same CSR with the mirrored bits
-        ctx.A, ctx.L, ctx.drop = A, n_layers, drop
+        # by its transpose, which is the same CSR with the mirrored bits.  div: the divisor of the last epilogue, L + 1 (the
+        # layer mean) unless given; 1 gives the plain sum E_0 + ... + E_L
+        div = float(n_layers + 1) if div is None else float(div)
+        ctx.A, ctx.L, ctx.drop, ctx.div = A, n_layers, drop, div
         ego = _f32c(ego)
         if n_layers == 0:
             return ego.clone()
@@ -435,16 +437,16 @@ class _PropagateMeanFn(torch.autograd.Function):
         for l in range(1, n_layers + 1):
             last = l == n_layers
             y = None if last else torch.empty_like(ego)
-            spmm_raw(A, x, Y=y, acc_in=ego if l == 1 else acc, acc_out=acc, acc_div=float(n_layers + 1) if last else 1.0, drop=fwd)
+            spmm_raw(A, x, Y=y, acc_in=ego if l == 1 else acc, acc_out=acc, acc_div=div if last else 1.0, drop=fwd)
             x = y
         return acc
 
     @staticmethod
     def backward(ctx, g):
         L = ctx.L
-        gm = _f32c(g) / float(L + 1)                # d mean / d E_l, the same for every layer
+        gm = _f32c(g) if ctx.div == 1.0 else _f32c(g) / ctx.div      # d out / d E_l, the same for every layer
         if L == 0:
-            return g, None, None, None
+            return g, None, None, None, None
         drop = ctx.drop
         At = ctx.A.t() if drop is None else ctx.A
         bwd = None if drop is None else (drop[1], drop[2])
@@ -453,7 +455,7 @@ class _PropagateMeanFn(torch.autograd.Function):
             nxt = torch.empty_like(gm)
             spmm_raw(At, cur, acc_in=gm, acc_out=nxt, drop=bwd)
             cur = nxt
-        return cur, None, None, None
+        return cur, None, None, None, None
 
 
 def propagate_mean(A: CSR, ego: torch.Tensor, n_layers: int) -> torch.Tensor:
@@ -461,6 +463,14 @@ def propagate_mean(A: CSR, ego: torch.Tensor, n_layers: int) -> torch.Tensor:
     (`src/models/freedom.py:169-176`, `bm3.py:86-92`, `lightgcn.py:116-123`, `mgcn.py:159-166`), with the
     running sum and the final division fused into the SpMM epilogue (no stack, no extra passes)."""
     return _PropagateMeanFn.apply(ego, A, n_layers)
+
+
+def propagate_sum(A: CSR, ego: torch.Tensor, n_layers: int) -> torch.Tensor:
+    """E_0 + E_1 + ... + E_L, E_{l+1} = A E_l: `propagate_mean` with 1 as the final divisor, so the running sum in the
+    SpMM epilogue is the whole result.  DualGNN's tower (`src/models/dualgnn.py:311-314`: `h = conv(x)`, `h_1 = conv(h)`,
+    `x_hat = h + x + h_1`) is L = 2: the first epilogue forms x + h, the second (x + h) + h_1, the reference's order of
+    additions.  Backward: g_l = g + A^T g_{l+1}."""
+    return _PropagateMeanFn.apply(ego, A, n_layers, None, 1.0)
 
 
 def edge_keep_bits(draws: torch.Tensor, keep_prob: float, draw_of: torch.Tensor, mirror: Optional[torch.Tensor] = None):

@@ -111,3 +111,44 @@ def write_dataset(root: str, name: str, g: SynthGraph, v_feat=None, t_feat=None,
     if t_feat is not None:
         np.save(os.path.join(d, "text_feat.npy"), t_feat)
     return d
+
+
+def user_graph_dict(g: SynthGraph, max_neighbours: int = 200, block: int = 1024) -> dict:
+    """The `user_graph_dict` of `preprocessing/dualgnn-gen-u-u-matrix.py` for `g` (DualGNN's user-user graph), without its
+    U(U-1)/2 Python set intersections and dense U x U matrix: per user, `[neighbours, counts]` of the users who share
+    training items with it (`x_label == 0`, each (user, item) pair counted once), best first, at most `max_neighbours`.
+
+    Counts are the binarised training matrix's co-occurrences R R^T, from scipy sparse products over `block` users at a
+    time, with the diagonal excluded (the script only counts pairs of distinct users).  Each user's row is then handed to
+    the script's own expression, `torch.topk` of the dense fp32 row with k = min(non-zeros, max_neighbours), so ties come
+    out in the script's order.  The script's U is the number of distinct users in the whole file."""
+    import scipy.sparse as sp
+    import torch
+    n_users = int(np.unique(g.user).size)
+    u, i = g.train
+    n_items = int(g.item.max()) + 1 if g.item.size else 0
+    R = sp.csr_matrix((np.ones(u.size, dtype=np.int64), (u, i)), shape=(n_users, n_items))
+    R.sum_duplicates()
+    R.data[:] = 1
+    Rt = R.T.tocsr()
+    out = {}
+    for lo in range(0, n_users, block):
+        hi = min(n_users, lo + block)
+        C = np.asarray((R[lo:hi] @ Rt).todense(), dtype=np.float32)
+        C[np.arange(hi - lo), np.arange(lo, hi)] = 0.0
+        T = torch.from_numpy(C)
+        nz = np.count_nonzero(C, axis=1)
+        for r in range(hi - lo):
+            top = torch.topk(T[r], int(min(nz[r], max_neighbours)))
+            out[lo + r] = [top.indices.numpy().tolist(), top.values.numpy().tolist()]
+    return out
+
+
+def write_user_graph_dict(root: str, name: str, g: SynthGraph, file_name: str = "user_graph_dict.npy", **kw) -> str:
+    """Write `<root>/<name>/<file_name>` (`user_graph_dict_file` of the dataset yaml) as the reference's preprocessing
+    script does: `np.save` of the pickled dict of `user_graph_dict(g)`."""
+    d = os.path.join(root, name)
+    os.makedirs(d, exist_ok=True)
+    path = os.path.join(d, file_name)
+    np.save(path, user_graph_dict(g, **kw), allow_pickle=True)
+    return path
