@@ -33,7 +33,7 @@ extern "C" {
 #define MMREC_ECUDA (-3)       /* a CUDA runtime call failed; see mmrec_last_error() */
 #define MMREC_EUNSUPPORTED (-4)/* device is not sm_90 (the library carries sm_90a code only) */
 
-#define MMREC_ABI_VERSION 3
+#define MMREC_ABI_VERSION 4
 
 int mmrec_abi_version(void);
 const char* mmrec_last_error(void);
@@ -60,7 +60,7 @@ int mmrec_csr_from_coo(int64_t nnz, const int64_t* row, const int64_t* col, cons
                        int32_t* rowptr, int32_t* colidx, float* vals, int64_t* nnz_out,
                        void* ws, size_t ws_bytes, void* stream);
 
-/* Work plan for mmrec_spmm_f32.  A task is a whole row or, for rows longer than `seg` non-zeros, one segment of it.
+/* Work plan for mmrec_spmm_run_f32.  A task is a whole row or, for rows longer than `seg` non-zeros, one segment of it.
  * Tasks longer than `light_max` are run by a whole CTA (its lane groups split the task and reduce through shared
  * memory), the others by one lane group each -- the power-law item rows neither serialise on one warp nor sit on
  * the critical path.
@@ -89,101 +89,79 @@ int mmrec_bipartite_norm_f32(int64_t n_edges, const int64_t* users, const int64_
  * lightgcn.py:115-128, mgcn.py:157-185, layergcn.py:125-138); its backward is the same call on the
  * transposed CSR (autograd of torch.sparse.mm, triggered at src/common/trainer.py:185).
  *
- *   y[r,:]   = sum_j vals[j] * X[colidx[j], :]           j in rowptr[r] .. rowptr[r+1]
- *   if gate_ref: y[r,:] *= cos(y[r,:], gate_ref[r,:])    (LayerGCN, layergcn.py:132-133)
- *   if Y:        Y[r,:] = y[r,:]
- *   if acc_out:  acc_out[r,:] = ((acc_in ? acc_in[r,:] : 0) + y[r,:]) / acc_div
+ * One mmrec_spmm_op describes one product of the n_rows x n_cols CSR (rowptr, colidx, vals) with X, d columns wide:
  *
- * acc_in may alias acc_out.  d in {32, 64, 128, 256} runs the vectorised kernel, any other d >= 1
- * the generic one.  d in {96, 192, 384} = 3 x {32, 64, 128} (several d-wide operands side by side,
- * SLMRec's three views) also runs the vectorised kernel, three float4 per lane on the lanes the width
- * d/3 uses: without the gate, every d/3-wide column block of the result is bit-identical to the
- * width-d/3 product of that block.  The lane override does not apply to these widths.  tasks/n_tasks/n_cta_tasks/split_rows/counters/partial come from mmrec_spmm_plan
- * (counters: int32[n_split_rows], zero on entry and zero again on exit; partial:
- * fp32[n_slots * d]); tasks == NULL selects one warp per row.  Summation order is fixed, so the
- * result is bit-reproducible run to run.
+ *   y[r,:]   = sum_j w_j * X[colidx[j], :]               j in rowptr[r] .. rowptr[r+1], w_j = vals[j]
+ *   if keep_bits: only the entries whose keep bit is set take part, w_j = fl(vals[j] * keep_scale)
+ *   if gate_ref:  y[r,:] *= cos(y[r,:], gate_ref[r,:])   (LayerGCN, layergcn.py:132-133)
+ *   if Y:         Y[r,:] = y[r,:]  (y_accumulate != 0: Y[r,:] += y[r,:])
+ *   if acc_out:   acc_out[r,:] = ((acc_in ? acc_in[r,:] : 0) + y[r,:]) / acc_div
+ *                 (+ post[r - post_row0,:] for r >= post_row0 when post is set, after the division)
+ *
+ *  - acc_in may alias acc_out.  Every matrix is row-major with the leading dimension beside it (in floats, >= d).
+ *  - Work plan: tasks/n_tasks/n_cta_tasks/split_rows/counters/partial come from mmrec_spmm_plan (counters:
+ *    int32[n_split_rows], zero on entry and zero again on exit; partial: fp32[n_slots * d]); tasks == NULL selects one
+ *    warp per row.  Summation order is fixed, so the result is bit-reproducible run to run.
+ *  - y_accumulate: for graphs whose X does not fit the L2 the matrix is cut into column panels whose share of X does; the
+ *    panels are multiplied one after the other and add up in Y, so every row of X is fetched from HBM once per layer
+ *    instead of once per non-zero (ops.PanelCSR).  The running-sum epilogue sees one panel's y only, so the division
+ *    belongs to the last panel.  Not with the gate (MMREC_EINVAL).
+ *  - keep_bits uint32[ceil(nnz / 32)], bit e (word e / 32, bit e % 32) for CSR position e (mmrec_edge_keep_bits):
+ *    `torch.sparse.mm(sparse_dropout(A, rate), X)` of src/common/encoders.py:77-88,99 without building the dropped matrix.
+ *    A dropped entry loads nothing and adds nothing, so the result equals the product with the compacted matrix and the
+ *    values fl(v * keep_scale), up to the position of the segment boundaries of split rows.  d in {32, 64, 128, 256} and
+ *    16-byte aligned operands, and neither the gate nor y_accumulate, else MMREC_EUNSUPPORTED.
+ *  - Second row blocks (nullable): X row c is X_hi[c - x_split, :] for c >= x_split, acc_in row r is
+ *    acc_in_hi[r - acc_in_split, :] for r >= acc_in_split (acc_in and acc_out must be set) -- layer 1 of a propagation
+ *    reads [users; items] straight from the two embedding tables, with the same bits as from their concatenation.
+ *
+ * mmrec_spmm_run_f32 runs n_ops products in order on `stream`.
+ *  - One op without X_hi, acc_in_hi, post or sync_before, cooperative == 0: with keep_bits, the masked kernel.  Otherwise
+ *    d in {32, 64, 128, 256} with 16-byte aligned operands runs the vectorised kernel (the lane override applies), as do
+ *    d in {96, 192, 384} = 3 x {32, 64, 128} (several d-wide operands side by side, SLMRec's three views: three float4
+ *    per lane on the lanes the width d/3 uses; without the gate, every d/3-wide column block of the result is
+ *    bit-identical to the width-d/3 product of that block; no lane override).  Any other d >= 1 or alignment runs the
+ *    generic kernel.
+ *  - Otherwise the ops are the SpMMs of one propagation (src/models/freedom.py:164-178: n_ui_layers products with A_hat,
+ *    the item-item product, the layer mean and `+ h`), at most 8, run by the chained kernel: every op needs its work
+ *    plan; d in {32, 64, 128, 256}, 16-byte aligned operands, no lane override, no gate, keep bits or y_accumulate --
+ *    otherwise MMREC_EUNSUPPORTED and the caller runs the ops one by one.  cooperative != 0: one persistent cooperative
+ *    launch, the ops run in order on one resident grid with a grid-wide barrier before every op whose `sync_before` is
+ *    set (= it reads what an earlier op wrote).  cooperative == 0: the ops up to the next `sync_before` op share one
+ *    ordinary launch (ops that do not read each other's output, such as FREEDOM's item-item product and layer 1 on
+ *    A_hat); each `sync_before` op starts a new launch on the stream.  Ops of one launch must not share a work plan's
+ *    counters / partial buffer.
  * ------------------------------------------------------------------------------------------- */
 /* tuning knob: lanes that cooperate on one row (0 = default min(32, d/4); a power of two, d/(4*lanes) float4 per lane;
  * d in {32, 64, 128, 256} only) */
 int mmrec_spmm_set_lanes(int lanes_per_row);
-int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d,
-                   const int32_t* rowptr, const int32_t* colidx, const float* vals,
-                   const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks, const int32_t* split_rows,
-                   int32_t* counters, float* partial,
-                   const float* X, int64_t ldx,
-                   float* Y, int64_t ldy,
-                   const float* acc_in, float* acc_out, int64_t ldacc, float acc_div,
-                   const float* gate_ref, int64_t ldgate,
-                   void* stream);
-
-/* mmrec_spmm_f32 without the gate and with an ACCUMULATING Y (y_accumulate != 0: Y[r,:] += y[r,:]; the running-sum epilogue
- * sees this call's y only, so the division belongs to the last call).  For graphs whose dense operand X does not fit the L2:
- * the matrix is cut into column panels whose share of X does, the panels are multiplied one after the other and add up in Y
- * -- every row of X is fetched from HBM once per layer instead of once per non-zero (ops.PanelCSR). */
-int mmrec_spmm_acc_f32(int64_t n_rows, int64_t n_cols, int d,
-                       const int32_t* rowptr, const int32_t* colidx, const float* vals,
-                       const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks, const int32_t* split_rows,
-                       int32_t* counters, float* partial,
-                       const float* X, int64_t ldx, float* Y, int64_t ldy,
-                       const float* acc_in, float* acc_out, int64_t ldacc, float acc_div, int y_accumulate, void* stream);
-
-/* mmrec_spmm_f32 (no gate) over the entries of the CSR whose keep bit is set, each weighted fl(vals[e] * scale):
- * `torch.sparse.mm(sparse_dropout(A, rate), X)` of src/common/encoders.py:77-88,99 without building the dropped matrix.
- * keep_bits uint32[ceil(nnz / 32)], bit e (word e / 32, bit e % 32) for CSR position e (mmrec_edge_keep_bits).  A dropped
- * entry loads nothing and adds nothing; the plan, split rows, segment-order reduction and epilogues are mmrec_spmm_f32's,
- * so the result equals mmrec_spmm_f32 on the compacted matrix with the values fl(v * scale), up to the position of the
- * segment boundaries of split rows.  d in {32, 64, 128, 256}, 16-byte aligned operands, else MMREC_EUNSUPPORTED. */
-int mmrec_spmm_drop_f32(int64_t n_rows, int64_t n_cols, int d,
-                        const int32_t* rowptr, const int32_t* colidx, const float* vals,
-                        const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks, const int32_t* split_rows,
-                        int32_t* counters, float* partial,
-                        const float* X, int64_t ldx, float* Y, int64_t ldy,
-                        const float* acc_in, float* acc_out, int64_t ldacc, float acc_div,
-                        const uint32_t* keep_bits, float scale, void* stream);
+typedef struct {
+    int64_t n_rows, n_cols;
+    const int32_t* rowptr; const int32_t* colidx; const float* vals;
+    const int32_t* tasks; int64_t n_tasks, n_cta_tasks;              /* tasks == NULL: one warp per row */
+    const int32_t* split_rows; int32_t* counters; float* partial;
+    const float* X; int64_t ldx;
+    const float* X_hi; int64_t ldx_hi, x_split;                      /* nullable: second row block of X */
+    float* Y; int64_t ldy; int y_accumulate;                         /* Y nullable */
+    const float* acc_in; float* acc_out; int64_t ldacc; float acc_div;
+    const float* acc_in_hi; int64_t ldacc_in_hi, acc_in_split;       /* nullable */
+    const float* gate_ref; int64_t ldgate;                           /* nullable: LayerGCN's cosine gate */
+    const float* post; int64_t ldpost, post_row0;                    /* nullable */
+    const uint32_t* keep_bits; float keep_scale;                     /* nullable: edge-keep mask */
+    int sync_before;
+} mmrec_spmm_op;
+int mmrec_spmm_run_f32(int d, int n_ops, const mmrec_spmm_op* ops, int cooperative, void* stream);
 
 /* The keep bits of one `sparse_dropout` draw (src/common/encoders.py:77-88): draw j of `torch.rand(nnz)` belongs to the
  * reference's j-th stored entry, which is CSR position e with draw_of[e] = j.  Position e is kept iff
  * floorf(keep_prob + draws[draw_of[e]]) != 0, one IEEE fp32 add (keep_prob = float32(1 - rate), as torch adds it).
- *   keep_bits   uint32[ceil(nnz / 32)]  the forward's bits, CSR order (mmrec_spmm_drop_f32)
+ *   keep_bits   uint32[ceil(nnz / 32)]  the forward's bits, CSR order (mmrec_spmm_op.keep_bits)
  *   mirror      int32[nnz] (nullable)   position of (c, r) for the entry (r, c) of a structurally symmetric CSR
  *   keep_bits_t uint32[ceil(nnz / 32)]  (nullable, needs mirror) bit e = bit mirror[e] of keep_bits: the dropped matrix's
  *                                       transpose on the same CSR when its values are symmetric (the backward)
  * Bits past nnz in the last word are 0. */
 int mmrec_edge_keep_bits(int64_t nnz, const float* draws, float keep_prob, const int32_t* draw_of, const int32_t* mirror,
                          uint32_t* keep_bits, uint32_t* keep_bits_t, void* stream);
-
-/* The SpMMs of one propagation as ONE persistent cooperative launch (src/models/freedom.py:164-178: n_ui_layers products with
- * A_hat, the item-item product, the layer mean and `+ h`): the steps run in order on one resident grid, with a grid-wide
- * barrier before every step whose `sync_before` is set (= it reads what an earlier step wrote).  Every step needs its work
- * plan; d in {32, 64, 128, 256}, 16-byte aligned operands -- otherwise MMREC_EUNSUPPORTED and the caller launches the steps
- * one by one with mmrec_spmm_f32.  Extra epilogue term: acc_out[r,:] += post[r - post_row0,:] for r >= post_row0, applied
- * after the division (FREEDOM's `i_g_embeddings + h`, freedom.py:178). */
-typedef struct {
-    int64_t n_rows, n_cols;
-    const int32_t* rowptr; const int32_t* colidx; const float* vals;
-    const int32_t* tasks; int64_t n_tasks, n_cta_tasks; const int32_t* split_rows; int32_t* counters; float* partial;
-    const float* X; int64_t ldx;
-    float* Y; int64_t ldy;                                   /* nullable */
-    const float* acc_in; float* acc_out; int64_t ldacc; float acc_div;   /* as mmrec_spmm_f32 */
-    const float* post; int64_t ldpost; int64_t post_row0;    /* nullable */
-    int sync_before;
-} mmrec_spmm_step;
-int mmrec_spmm_chain_f32(int d, int n_steps, const mmrec_spmm_step* steps, void* stream);
-
-/* The general form: mmrec_spmm_chain_f32 is this call with cooperative = 1 and no second blocks.
- *   Second row blocks of the dense operands (nullable): X row c is X_hi[c - x_split, :] for c >= x_split, acc_in row r is
- *   acc_in_hi[r - acc_in_split, :] for r >= acc_in_split (acc_in and acc_out must be set) -- layer 1 of a propagation reads
- *   [users; items] straight from the two embedding tables, with the same bits as from their concatenation.
- *   cooperative != 0: one cooperative launch, a grid barrier before every `sync_before` step.  cooperative == 0: the steps up
- *   to the next `sync_before` step share one ordinary launch (steps that do not read each other's output, such as FREEDOM's
- *   item-item product and layer 1 on A_hat); each `sync_before` step starts a new launch on the stream.  Steps of one launch
- *   must not share a work plan's counters / partial buffer. */
-typedef struct {
-    mmrec_spmm_step step;
-    const float* X_hi; int64_t ldx_hi; int64_t x_split;                   /* nullable */
-    const float* acc_in_hi; int64_t ldacc_in_hi; int64_t acc_in_split;    /* nullable */
-} mmrec_spmm_step2;
-int mmrec_spmm_steps_f32(int d, int n_steps, const mmrec_spmm_step2* steps, int cooperative, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * K2  fused gather -> linear(+bias) -> optional row L2-normalise.   Replaces

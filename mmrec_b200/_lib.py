@@ -26,15 +26,8 @@ PROTOTYPES = {
     "mmrec_bipartite_norm_workspace_bytes": (_sz, [_i64, _i64]),
     "mmrec_bipartite_norm_f32": (_i32, [_i64, _p, _p, _i64, _i64, _f32, _p, _p, _sz, _p]),
     "mmrec_spmm_set_lanes": (_i32, [_i32]),
-    "mmrec_spmm_f32": (_i32, [_i64, _i64, _i32, _p, _p, _p, _p, _i64, _i64, _p, _p, _p, _p, _i64, _p, _i64, _p, _p, _i64,
-                              _f32, _p, _i64, _p]),
-    "mmrec_spmm_acc_f32": (_i32, [_i64, _i64, _i32, _p, _p, _p, _p, _i64, _i64, _p, _p, _p, _p, _i64, _p, _i64, _p, _p, _i64,
-                                  _f32, _i32, _p]),
-    "mmrec_spmm_drop_f32": (_i32, [_i64, _i64, _i32, _p, _p, _p, _p, _i64, _i64, _p, _p, _p, _p, _i64, _p, _i64, _p, _p, _i64,
-                                   _f32, _p, _f32, _p]),
+    "mmrec_spmm_run_f32": (_i32, [_i32, _i32, _p, _i32, _p]),
     "mmrec_edge_keep_bits": (_i32, [_i64, _p, _f32, _p, _p, _p, _p, _p]),
-    "mmrec_spmm_chain_f32": (_i32, [_i32, _i32, _p, _p]),
-    "mmrec_spmm_steps_f32": (_i32, [_i32, _i32, _p, _i32, _p]),
     "mmrec_project_set_path": (_i32, [_i32]),
     "mmrec_project_workspace_bytes": (_sz, [_i64, _i64, _i32]),
     "mmrec_project_f32": (_i32, [_i64, _p, _p, _i64, _i64, _p, _p, _i32, _i32, _p, _i64, _p, _sz, _p]),
@@ -85,19 +78,16 @@ PROTOTYPES = {
     "mmrec_mgcn_fuse_f32": (_i32, [_i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
 }
 
-class SpmmStep(C.Structure):
-    """`mmrec_spmm_step` of include/mmrec_b200.h."""
+class SpmmOp(C.Structure):
+    """`mmrec_spmm_op` of include/mmrec_b200.h."""
     _fields_ = [("n_rows", _i64), ("n_cols", _i64), ("rowptr", _p), ("colidx", _p), ("vals", _p),
                 ("tasks", _p), ("n_tasks", _i64), ("n_cta_tasks", _i64), ("split_rows", _p), ("counters", _p), ("partial", _p),
-                ("X", _p), ("ldx", _i64), ("Y", _p), ("ldy", _i64),
+                ("X", _p), ("ldx", _i64), ("X_hi", _p), ("ldx_hi", _i64), ("x_split", _i64),
+                ("Y", _p), ("ldy", _i64), ("y_accumulate", _i32),
                 ("acc_in", _p), ("acc_out", _p), ("ldacc", _i64), ("acc_div", _f32),
-                ("post", _p), ("ldpost", _i64), ("post_row0", _i64), ("sync_before", _i32)]
-
-
-class SpmmStep2(C.Structure):
-    """`mmrec_spmm_step2` of include/mmrec_b200.h: a step plus the second row blocks of X and acc_in."""
-    _fields_ = [("step", SpmmStep), ("X_hi", _p), ("ldx_hi", _i64), ("x_split", _i64),
-                ("acc_in_hi", _p), ("ldacc_in_hi", _i64), ("acc_in_split", _i64)]
+                ("acc_in_hi", _p), ("ldacc_in_hi", _i64), ("acc_in_split", _i64),
+                ("gate_ref", _p), ("ldgate", _i64), ("post", _p), ("ldpost", _i64), ("post_row0", _i64),
+                ("keep_bits", _p), ("keep_scale", _f32), ("sync_before", _i32)]
 
 
 class AdamTensor(C.Structure):
@@ -106,7 +96,7 @@ class AdamTensor(C.Structure):
 
 
 _lib = None
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 class MMRecError(RuntimeError):

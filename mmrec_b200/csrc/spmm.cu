@@ -35,7 +35,7 @@ struct SpmmParams {
     const float* post; int64_t post_row0; uint32_t spost;   // acc_out[r,:] += post[r - post_row0, :] for r >= post_row0 (after the division)
     int d;
     uint32_t sx, sy, sacc, sgate;      // the leading dimensions as byte strides (vector kernel: one IMAD.WIDE per row address)
-    // Two-block operands (chained kernel only, mmrec_spmm_steps_f32): row c of X is X_hi[c - x_split] for c >= x_split, row r of
+    // Two-block operands (chained kernel only, mmrec_spmm_op.X_hi): row c of X is X_hi[c - x_split] for c >= x_split, row r of
     // acc_in is acc_in_hi[r - acc_split] for r >= acc_split -- [users; items] straight from the two embedding tables, no copy.
     // One block: X_hi = X, x_split = n_cols, acc_in_hi = acc_in, acc_split = n_rows.
     const float* X_hi; const float* acc_in_hi;
@@ -365,7 +365,7 @@ __global__ void __launch_bounds__(256) spmm_vec_kernel(const SpmmParams p) {
     spmm_vec_body<D, T, false>(p, red);
 }
 
-// K1 with an edge-keep mask (mmrec_spmm_drop_f32): the same plan, split rows, segment-order reduction and epilogues, over
+// K1 with an edge-keep mask (mmrec_spmm_op.keep_bits): the same plan, split rows, segment-order reduction and epilogues, over
 // the entries whose keep bit is set, each weighted fl(v * scale) -- SelfCF's per-batch `sparse_dropout` of the normalised
 // adjacency (encoders.py:77-88) without rebuilding the matrix.
 template <int D, int T>
@@ -450,7 +450,6 @@ __global__ void __launch_bounds__(256) spmm_generic_kernel(const SpmmParams p) {
     }
 }
 
-static thread_local int g_spmm_y_acc = 0;   // set by mmrec_spmm_acc_f32 around its call of mmrec_spmm_f32
 int g_spmm_lanes = 0;   // 0 = default lanes per task for the width; set by mmrec_spmm_set_lanes (tuning knob)
 
 template <int D, int T, bool DROP = false>
@@ -507,97 +506,6 @@ extern "C" int mmrec_spmm_set_lanes(int lanes_per_row) {
     return MMREC_OK;
 }
 
-namespace mmrec {
-// The argument checks and parameter block shared by mmrec_spmm_f32 and mmrec_spmm_drop_f32; sets *vec_ok when the operands
-// are 16-byte aligned (the vector kernel's float4 rows).
-static int spmm_params(SpmmParams& p, bool& vec_ok, int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
-                       const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks, const int32_t* split_rows,
-                       int32_t* counters, float* partial, const float* X, int64_t ldx, float* Y, int64_t ldy, const float* acc_in,
-                       float* acc_out, int64_t ldacc, float acc_div, const float* gate_ref, int64_t ldgate) {
-    MMREC_CHECK_ARG(rowptr && X && (Y || acc_out), "spmm: null pointer");
-    MMREC_CHECK_ARG(ldx >= d && (!Y || ldy >= d) && (!acc_out || ldacc >= d) && (!gate_ref || ldgate >= d), "spmm: leading dimension < d");
-    MMREC_CHECK_ARG(acc_div != 0.0f, "spmm: acc_div == 0");
-    MMREC_CHECK_ARG(!tasks || (n_tasks >= 0 && n_cta_tasks >= 0 && n_cta_tasks <= n_tasks && split_rows && counters && partial),
-                    "spmm: plan pointers missing");
-    p.n_rows = n_rows; p.n_cols = n_cols; p.rowptr = rowptr; p.colidx = colidx; p.vals = vals;
-    p.tasks = (const int4*)tasks; p.n_tasks = n_tasks; p.n_heavy = tasks ? n_cta_tasks : 0; p.split_rows = (const int4*)split_rows;
-    p.counters = counters; p.partial = partial; p.X = X; p.ldx = ldx; p.Y = Y; p.ldy = ldy;
-    p.acc_in = acc_in; p.acc_out = acc_out; p.ldacc = ldacc; p.acc_div = acc_div; p.gate_ref = gate_ref;
-    p.ldgate = ldgate; p.d = d;
-    p.post = nullptr; p.post_row0 = 0; p.spost = 0; p.y_acc = g_spmm_y_acc;
-    MMREC_CHECK_ARG(!(p.y_acc && gate_ref), "spmm: y_accumulate does not combine with the cosine gate");
-    MMREC_CHECK_ARG(ldx < (1ll << 30) && ldy < (1ll << 30) && ldacc < (1ll << 30) && ldgate < (1ll << 30) && n_cols < (1ll << 31) &&
-                    n_rows < (1ll << 31), "spmm: leading dimension / size out of range");
-    p.sx = (uint32_t)(ldx * 4); p.sy = (uint32_t)(ldy * 4); p.sacc = (uint32_t)(ldacc * 4); p.sgate = (uint32_t)(ldgate * 4);
-    p.X_hi = X; p.x_split = (int)n_cols; p.sx_hi = p.sx; p.acc_in_hi = acc_in; p.acc_split = (int)n_rows; p.sacc_hi = p.sacc;
-    auto al16 = [](const void* q, int64_t ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld & 3) == 0); };
-    vec_ok = al16(X, ldx) && al16(Y, ldy) && al16(acc_in, ldacc) && al16(acc_out, ldacc) && al16(gate_ref, ldgate) && al16(partial, 4);
-    return MMREC_OK;
-}
-}  // namespace mmrec
-
-extern "C" int mmrec_spmm_f32(int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
-                              const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks,
-                              const int32_t* split_rows,
-                              int32_t* counters, float* partial, const float* X, int64_t ldx, float* Y, int64_t ldy,
-                              const float* acc_in, float* acc_out, int64_t ldacc, float acc_div, const float* gate_ref,
-                              int64_t ldgate, void* stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    MMREC_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && d >= 1, "spmm: bad sizes");
-    if (n_rows == 0) return MMREC_OK;
-    SpmmParams p;
-    bool vec_ok = false;
-    const int rc = spmm_params(p, vec_ok, n_rows, n_cols, d, rowptr, colidx, vals, tasks, n_tasks, n_cta_tasks, split_rows, counters,
-                               partial, X, ldx, Y, ldy, acc_in, acc_out, ldacc, acc_div, gate_ref, ldgate);
-    if (rc != MMREC_OK) return rc;
-    if (vec_ok) {
-        switch (d) {
-            case 32: return launch_vec_d<32>(p, stream);
-            case 64: return launch_vec_d<64>(p, stream);
-            case 128: return launch_vec_d<128>(p, stream);
-            case 256: return launch_vec_d<256>(p, stream);
-            case 96: return launch_vec_3d<96>(p, stream);
-            case 192: return launch_vec_3d<192>(p, stream);
-            case 384: return launch_vec_3d<384>(p, stream);
-            default: break;
-        }
-    }
-    p.tasks = nullptr;   // the generic kernel walks whole rows
-    int64_t grid = (n_rows + 7) / 8;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (grid > cap) grid = cap;
-    spmm_generic_kernel<<<(unsigned)grid, 256, 0, stream>>>(p);
-    MMREC_LAUNCH_CHECK();
-    return MMREC_OK;
-}
-
-extern "C" int mmrec_spmm_drop_f32(int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
-                                   const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks,
-                                   const int32_t* split_rows, int32_t* counters, float* partial, const float* X, int64_t ldx,
-                                   float* Y, int64_t ldy, const float* acc_in, float* acc_out, int64_t ldacc, float acc_div,
-                                   const uint32_t* keep_bits, float scale, void* stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    MMREC_CHECK_ARG(n_rows >= 0 && n_cols >= 0 && d >= 1, "spmm_drop: bad sizes");
-    if (n_rows == 0) return MMREC_OK;
-    MMREC_CHECK_ARG(keep_bits, "spmm_drop: keep_bits is null");
-    SpmmParams p;
-    bool vec_ok = false;
-    const int rc = spmm_params(p, vec_ok, n_rows, n_cols, d, rowptr, colidx, vals, tasks, n_tasks, n_cta_tasks, split_rows, counters,
-                               partial, X, ldx, Y, ldy, acc_in, acc_out, ldacc, acc_div, nullptr, 0);
-    if (rc != MMREC_OK) return rc;
-    if (!vec_ok || !(d == 32 || d == 64 || d == 128 || d == 256)) {
-        set_error("spmm_drop: d = %d or unaligned operands: the masked kernel is built for 16-byte aligned d in {32, 64, 128, 256}", d);
-        return MMREC_EUNSUPPORTED;
-    }
-    const DropKeep dk{keep_bits, scale};
-    switch (d) {                                      // one float4 per lane, the default of the unmasked kernel
-        case 32: return launch_vec<32, 8, true>(p, stream, dk);
-        case 64: return launch_vec<64, 16, true>(p, stream, dk);
-        case 128: return launch_vec<128, 32, true>(p, stream, dk);
-        default: return launch_vec<256, 32, true>(p, stream, dk);
-    }
-}
-
 extern "C" int mmrec_edge_keep_bits(int64_t nnz, const float* draws, float keep_prob, const int32_t* draw_of, const int32_t* mirror,
                                     uint32_t* keep_bits, uint32_t* keep_bits_t, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -611,20 +519,6 @@ extern "C" int mmrec_edge_keep_bits(int64_t nnz, const float* draws, float keep_
     edge_keep_bits_kernel<<<(unsigned)grid, 256, 0, stream>>>(nnz, draws, keep_prob, draw_of, mirror, keep_bits, keep_bits_t);
     MMREC_LAUNCH_CHECK();
     return MMREC_OK;
-}
-
-// mmrec_spmm_f32 whose Y output ACCUMULATES (Y += A X): the column panels of one matrix are multiplied one after the other
-// so that the gathered rows of X stay L2-resident (graphs whose dense operand does not fit the L2).
-extern "C" int mmrec_spmm_acc_f32(int64_t n_rows, int64_t n_cols, int d, const int32_t* rowptr, const int32_t* colidx,
-                                  const float* vals, const int32_t* tasks, int64_t n_tasks, int64_t n_cta_tasks,
-                                  const int32_t* split_rows, int32_t* counters, float* partial, const float* X, int64_t ldx, float* Y,
-                                  int64_t ldy, const float* acc_in, float* acc_out, int64_t ldacc, float acc_div, int y_accumulate,
-                                  void* stream_) {
-    g_spmm_y_acc = y_accumulate ? 1 : 0;
-    const int rc = mmrec_spmm_f32(n_rows, n_cols, d, rowptr, colidx, vals, tasks, n_tasks, n_cta_tasks, split_rows, counters, partial, X, ldx,
-                                  Y, ldy, acc_in, acc_out, ldacc, acc_div, nullptr, 0, stream_);
-    g_spmm_y_acc = 0;
-    return rc;
 }
 
 namespace mmrec {
@@ -682,64 +576,120 @@ static int launch_steps(const SpmmChain& c, int cooperative, cudaStream_t stream
     }
     return MMREC_OK;
 }
+
+// The checks of one op and its parameter block.  chain: the chained kernel's limits (every op needs its work plan).  Sets
+// vec_ok when the operands are 16-byte aligned (the vector kernels' float4 rows).
+static int spmm_op_params(const mmrec_spmm_op& o, int i, int d, bool chain, SpmmParams& p, bool& vec_ok) {
+    MMREC_CHECK_ARG(o.n_rows >= 0 && o.n_cols >= 0 && o.rowptr && o.X && (o.Y || o.acc_out), "spmm: op %d: null pointer / bad sizes", i);
+    MMREC_CHECK_ARG(o.tasks ? (o.n_tasks >= 0 && o.n_cta_tasks >= 0 && o.n_cta_tasks <= o.n_tasks && o.split_rows && o.counters && o.partial)
+                            : !chain,
+                    "spmm: op %d: work plan pointers missing (the chained kernel needs the plan of mmrec_spmm_plan)", i);
+    MMREC_CHECK_ARG(o.ldx >= d && (!o.Y || o.ldy >= d) && (!o.acc_out || o.ldacc >= d) && (!o.gate_ref || o.ldgate >= d) &&
+                    (!o.post || o.ldpost >= d) && o.acc_div != 0.0f, "spmm: op %d: leading dimension < d or acc_div == 0", i);
+    MMREC_CHECK_ARG(!(o.y_accumulate && o.gate_ref), "spmm: y_accumulate does not combine with the cosine gate");
+    MMREC_CHECK_ARG(o.ldx < (1ll << 30) && o.ldy < (1ll << 30) && o.ldacc < (1ll << 30) && o.ldgate < (1ll << 30) && o.ldpost < (1ll << 30) &&
+                    o.n_cols < (1ll << 31) && o.n_rows < (1ll << 31), "spmm: op %d: leading dimension / size out of range", i);
+    MMREC_CHECK_ARG(!o.X_hi || (o.x_split >= 0 && o.x_split <= o.n_cols && o.ldx_hi >= d && o.ldx_hi < (1ll << 30)),
+                    "spmm: op %d: X_hi needs 0 <= x_split <= n_cols and d <= ldx_hi < 2^30", i);
+    MMREC_CHECK_ARG(!o.acc_in_hi || (o.acc_in && o.acc_out && o.acc_in_split >= 0 && o.acc_in_split <= o.n_rows && o.ldacc_in_hi >= d &&
+                                     o.ldacc_in_hi < (1ll << 30)),
+                    "spmm: op %d: acc_in_hi needs acc_in, acc_out, 0 <= acc_in_split <= n_rows and d <= ldacc_in_hi < 2^30", i);
+    p.n_rows = o.n_rows; p.n_cols = o.n_cols; p.rowptr = o.rowptr; p.colidx = o.colidx; p.vals = o.vals;
+    p.tasks = (const int4*)o.tasks; p.n_tasks = o.n_tasks; p.n_heavy = o.tasks ? o.n_cta_tasks : 0; p.split_rows = (const int4*)o.split_rows;
+    p.counters = o.counters; p.partial = o.partial; p.X = o.X; p.ldx = o.ldx; p.Y = o.Y; p.ldy = o.ldy; p.y_acc = o.y_accumulate != 0;
+    p.acc_in = o.acc_in; p.acc_out = o.acc_out; p.ldacc = o.ldacc; p.acc_div = o.acc_div; p.gate_ref = o.gate_ref; p.ldgate = o.ldgate;
+    p.post = o.post; p.post_row0 = o.post_row0; p.d = d;
+    p.sx = (uint32_t)(o.ldx * 4); p.sy = (uint32_t)(o.ldy * 4); p.sacc = (uint32_t)(o.ldacc * 4); p.sgate = (uint32_t)(o.ldgate * 4);
+    p.spost = (uint32_t)(o.ldpost * 4);
+    p.X_hi = o.X_hi ? o.X_hi : o.X;
+    p.x_split = (int)(o.X_hi ? o.x_split : o.n_cols);
+    p.sx_hi = (uint32_t)((o.X_hi ? o.ldx_hi : o.ldx) * 4);
+    p.acc_in_hi = o.acc_in_hi ? o.acc_in_hi : o.acc_in;
+    p.acc_split = (int)(o.acc_in_hi ? o.acc_in_split : o.n_rows);
+    p.sacc_hi = (uint32_t)((o.acc_in_hi ? o.ldacc_in_hi : o.ldacc) * 4);
+    auto al16 = [](const void* q, int64_t ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld & 3) == 0); };
+    vec_ok = al16(o.X, o.ldx) && al16(o.Y, o.ldy) && al16(o.acc_in, o.ldacc) && al16(o.acc_out, o.ldacc) && al16(o.gate_ref, o.ldgate) &&
+             al16(o.post, o.ldpost) && al16(o.partial, 4) && al16(o.X_hi, o.ldx_hi) && al16(o.acc_in_hi, o.ldacc_in_hi);
+    return MMREC_OK;
+}
 }  // namespace mmrec
 
-extern "C" int mmrec_spmm_steps_f32(int d, int n_steps, const mmrec_spmm_step2* steps, int cooperative, void* stream_) {
+extern "C" int mmrec_spmm_run_f32(int d, int n_ops, const mmrec_spmm_op* ops, int cooperative, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
-    MMREC_CHECK_ARG(n_steps >= 1 && n_steps <= SPMM_CHAIN_MAX && steps, "spmm_steps: 1 <= n_steps <= %d", SPMM_CHAIN_MAX);
-    if (!(d == 32 || d == 64 || d == 128 || d == 256) || g_spmm_lanes) {
-        set_error("spmm_steps: d = %d (or a lane override) has no chained kernel; launch the steps one by one", d);
-        return MMREC_EUNSUPPORTED;
-    }
-    SpmmChain c;
-    c.n = n_steps; c.sync_mask = 0;
-    auto al16 = [](const void* q, int64_t ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld & 3) == 0); };
-    for (int i = 0; i < n_steps; ++i) {
-        const mmrec_spmm_step& t = steps[i].step;
-        const mmrec_spmm_step2& t2 = steps[i];
-        MMREC_CHECK_ARG(t.n_rows >= 0 && t.n_cols >= 0 && t.rowptr && t.X && (t.Y || t.acc_out), "spmm_steps: step %d: null pointer / bad sizes", i);
-        MMREC_CHECK_ARG(t.tasks && t.n_tasks >= 0 && t.n_cta_tasks >= 0 && t.n_cta_tasks <= t.n_tasks && t.split_rows && t.counters && t.partial,
-                        "spmm_steps: step %d: the chained kernel needs the work plan (mmrec_spmm_plan)", i);
-        MMREC_CHECK_ARG(t.ldx >= d && (!t.Y || t.ldy >= d) && (!t.acc_out || t.ldacc >= d) && (!t.post || t.ldpost >= d) && t.acc_div != 0.0f,
-                        "spmm_steps: step %d: leading dimension < d or acc_div == 0", i);
-        MMREC_CHECK_ARG(t.ldx < (1ll << 30) && t.ldy < (1ll << 30) && t.ldacc < (1ll << 30) && t.ldpost < (1ll << 30) && t.n_cols < (1ll << 31) &&
-                        t.n_rows < (1ll << 31), "spmm_steps: step %d: size out of range", i);
-        MMREC_CHECK_ARG(!t2.X_hi || (t2.x_split >= 0 && t2.x_split <= t.n_cols && t2.ldx_hi >= d && t2.ldx_hi < (1ll << 30)),
-                        "spmm_steps: step %d: X_hi needs 0 <= x_split <= n_cols and d <= ldx_hi < 2^30", i);
-        MMREC_CHECK_ARG(!t2.acc_in_hi || (t.acc_in && t.acc_out && t2.acc_in_split >= 0 && t2.acc_in_split <= t.n_rows && t2.ldacc_in_hi >= d &&
-                                          t2.ldacc_in_hi < (1ll << 30)),
-                        "spmm_steps: step %d: acc_in_hi needs acc_in, acc_out, 0 <= acc_in_split <= n_rows and d <= ldacc_in_hi < 2^30", i);
-        if (!(al16(t.X, t.ldx) && al16(t.Y, t.ldy) && al16(t.acc_in, t.ldacc) && al16(t.acc_out, t.ldacc) && al16(t.post, t.ldpost) && al16(t.partial, 4) &&
-              al16(t2.X_hi, t2.ldx_hi) && al16(t2.acc_in_hi, t2.ldacc_in_hi))) {
-            set_error("spmm_steps: step %d: operands not 16-byte aligned; launch the steps one by one", i);
+    MMREC_CHECK_ARG(n_ops >= 1 && n_ops <= SPMM_CHAIN_MAX && ops, "spmm: 1 <= n_ops <= %d", SPMM_CHAIN_MAX);
+    const bool vec_d = d == 32 || d == 64 || d == 128 || d == 256;
+    bool chain = n_ops > 1 || cooperative;
+    for (int i = 0; i < n_ops; ++i) chain = chain || ops[i].X_hi || ops[i].acc_in_hi || ops[i].post || ops[i].sync_before;
+    if (chain) {
+        if (!vec_d || g_spmm_lanes) {
+            set_error("spmm: d = %d (or a lane override) has no chained kernel; run the ops one by one", d);
             return MMREC_EUNSUPPORTED;
         }
-        SpmmParams& p = c.step[i];
-        p.n_rows = t.n_rows; p.n_cols = t.n_cols; p.rowptr = t.rowptr; p.colidx = t.colidx; p.vals = t.vals;
-        p.tasks = (const int4*)t.tasks; p.n_tasks = t.n_tasks; p.n_heavy = t.n_cta_tasks; p.split_rows = (const int4*)t.split_rows;
-        p.counters = t.counters; p.partial = t.partial; p.X = t.X; p.ldx = t.ldx; p.Y = t.Y; p.ldy = t.ldy;
-        p.acc_in = t.acc_in; p.acc_out = t.acc_out; p.ldacc = t.ldacc; p.acc_div = t.acc_div; p.gate_ref = nullptr; p.ldgate = 0;
-        p.post = t.post; p.post_row0 = t.post_row0; p.d = d; p.y_acc = 0;
-        p.sx = (uint32_t)(t.ldx * 4); p.sy = (uint32_t)(t.ldy * 4); p.sacc = (uint32_t)(t.ldacc * 4); p.sgate = 0; p.spost = (uint32_t)(t.ldpost * 4);
-        p.X_hi = t2.X_hi ? t2.X_hi : t.X;
-        p.x_split = (int)(t2.X_hi ? t2.x_split : t.n_cols);
-        p.sx_hi = (uint32_t)((t2.X_hi ? t2.ldx_hi : t.ldx) * 4);
-        p.acc_in_hi = t2.acc_in_hi ? t2.acc_in_hi : t.acc_in;
-        p.acc_split = (int)(t2.acc_in_hi ? t2.acc_in_split : t.n_rows);
-        p.sacc_hi = (uint32_t)((t2.acc_in_hi ? t2.ldacc_in_hi : t.ldacc) * 4);
-        if (t.sync_before && i > 0) c.sync_mask |= 1u << i;
+        SpmmChain c;
+        c.n = n_ops; c.sync_mask = 0;
+        for (int i = 0; i < n_ops; ++i) {
+            const mmrec_spmm_op& o = ops[i];
+            if (o.gate_ref || o.keep_bits || o.y_accumulate) {
+                set_error("spmm: op %d: the chained kernel has no cosine gate, edge-keep mask or accumulating Y", i);
+                return MMREC_EUNSUPPORTED;
+            }
+            bool vec_ok = false;
+            const int rc = spmm_op_params(o, i, d, true, c.step[i], vec_ok);
+            if (rc != MMREC_OK) return rc;
+            if (!vec_ok) {
+                set_error("spmm: op %d: operands not 16-byte aligned; run the ops one by one", i);
+                return MMREC_EUNSUPPORTED;
+            }
+            if (o.sync_before && i > 0) c.sync_mask |= 1u << i;
+        }
+        switch (d) {
+            case 32: return launch_steps<32>(c, cooperative, stream);
+            case 64: return launch_steps<64>(c, cooperative, stream);
+            case 128: return launch_steps<128>(c, cooperative, stream);
+            default: return launch_steps<256>(c, cooperative, stream);
+        }
     }
-    switch (d) {
-        case 32: return launch_steps<32>(c, cooperative, stream);
-        case 64: return launch_steps<64>(c, cooperative, stream);
-        case 128: return launch_steps<128>(c, cooperative, stream);
-        default: return launch_steps<256>(c, cooperative, stream);
+    const mmrec_spmm_op& o = ops[0];
+    MMREC_CHECK_ARG(o.n_rows >= 0 && o.n_cols >= 0 && d >= 1, "spmm: bad sizes");
+    if (o.n_rows == 0) return MMREC_OK;
+    if (o.keep_bits && (o.gate_ref || o.y_accumulate)) {
+        set_error("spmm: the edge-keep mask does not combine with the cosine gate or an accumulating Y");
+        return MMREC_EUNSUPPORTED;
     }
-}
-
-extern "C" int mmrec_spmm_chain_f32(int d, int n_steps, const mmrec_spmm_step* steps, void* stream_) {
-    MMREC_CHECK_ARG(n_steps >= 1 && n_steps <= SPMM_CHAIN_MAX && steps, "spmm_chain: 1 <= n_steps <= %d", SPMM_CHAIN_MAX);
-    mmrec_spmm_step2 s2[SPMM_CHAIN_MAX] = {};
-    for (int i = 0; i < n_steps; ++i) s2[i].step = steps[i];
-    return mmrec_spmm_steps_f32(d, n_steps, s2, 1, stream_);
+    SpmmParams p;
+    bool vec_ok = false;
+    const int rc = spmm_op_params(o, 0, d, false, p, vec_ok);
+    if (rc != MMREC_OK) return rc;
+    if (o.keep_bits) {
+        if (!vec_ok || !vec_d) {
+            set_error("spmm: d = %d or unaligned operands: the masked kernel is built for 16-byte aligned d in {32, 64, 128, 256}", d);
+            return MMREC_EUNSUPPORTED;
+        }
+        const DropKeep dk{o.keep_bits, o.keep_scale};
+        switch (d) {                                      // one float4 per lane, the default of the unmasked kernel
+            case 32: return launch_vec<32, 8, true>(p, stream, dk);
+            case 64: return launch_vec<64, 16, true>(p, stream, dk);
+            case 128: return launch_vec<128, 32, true>(p, stream, dk);
+            default: return launch_vec<256, 32, true>(p, stream, dk);
+        }
+    }
+    if (vec_ok) {
+        switch (d) {
+            case 32: return launch_vec_d<32>(p, stream);
+            case 64: return launch_vec_d<64>(p, stream);
+            case 128: return launch_vec_d<128>(p, stream);
+            case 256: return launch_vec_d<256>(p, stream);
+            case 96: return launch_vec_3d<96>(p, stream);
+            case 192: return launch_vec_3d<192>(p, stream);
+            case 384: return launch_vec_3d<384>(p, stream);
+            default: break;
+        }
+    }
+    p.tasks = nullptr;   // the generic kernel walks whole rows
+    int64_t grid = (o.n_rows + 7) / 8;
+    const int64_t cap = (int64_t)sm_count() * 8;
+    if (grid > cap) grid = cap;
+    spmm_generic_kernel<<<(unsigned)grid, 256, 0, stream>>>(p);
+    MMREC_LAUNCH_CHECK();
+    return MMREC_OK;
 }

@@ -7,6 +7,7 @@ sm_90 device, otherwise `MMRecError` is raised.
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Optional
 
 import torch
@@ -243,7 +244,7 @@ def spmm_raw(A, X: torch.Tensor, Y: Optional[torch.Tensor] = None, acc_in: Optio
     """y = A X with the fused epilogue of include/mmrec_b200.h (no autograd).  Replaces `torch.sparse.mm`
     (`src/models/freedom.py:167,172`) plus the stack/mean (`:175-176`) and `+ h` (`:178`) that follow.
     `drop` = (keep_bits, scale): only the entries whose keep bit is set take part, weighted fl(v * scale)
-    (`mmrec_spmm_drop_f32`; SelfCF's `sparse_dropout`, `src/common/encoders.py:77-88`)."""
+    (the edge-keep mask of `mmrec_spmm_op`; SelfCF's `sparse_dropout`, `src/common/encoders.py:77-88`)."""
     if drop is not None and (isinstance(A, PanelCSR) or gate_ref is not None or y_accumulate):
         raise MMRecError("spmm: the edge-keep mask runs on a CSR without the gate or y_accumulate")
     if isinstance(A, PanelCSR):
@@ -266,35 +267,39 @@ def spmm_raw(A, X: torch.Tensor, Y: Optional[torch.Tensor] = None, acc_in: Optio
             raise MMRecError(f"spmm: {name} must be contiguous float32 [{A.n_rows}, {d}]")
     if Y is None and acc_out is None:
         raise MMRecError("spmm: nothing to write")
-    plan = use_plan and A.n_tasks > 0
-    if y_accumulate:
-        if gate_ref is not None or Y is None:
-            raise MMRecError("spmm: y_accumulate needs Y and no gate")
-        check(lib.mmrec_spmm_acc_f32(A.n_rows, A.n_cols, d, _ptr(A.rowptr), _ptr(A.colidx), _ptr(A.vals),
-                                     _ptr(A.tasks) if plan else None, A.n_tasks if plan else 0, A.n_cta_tasks if plan else 0,
-                                     _ptr(A.split_rows) if plan else None, _ptr(A.counters) if plan else None,
-                                     _ptr(A.partial(d)) if plan else None,
-                                     _ptr(X), X.stride(0), _ptr(Y), d, _ptr(acc_in), _ptr(acc_out), d, float(acc_div), 1, _stream()),
-              "mmrec_spmm_acc_f32")
-        return
+    if y_accumulate and (gate_ref is not None or Y is None):
+        raise MMRecError("spmm: y_accumulate needs Y and no gate")
     if drop is not None:
-        keep, scale = drop
+        keep = drop[0]
         _need_cuda(keep)
         if keep.dtype != torch.int32 or not keep.is_contiguous() or keep.numel() < (A.nnz + 31) // 32:
             raise MMRecError("spmm: keep_bits must be contiguous int32 [ceil(nnz / 32)]")
-        check(lib.mmrec_spmm_drop_f32(A.n_rows, A.n_cols, d, _ptr(A.rowptr), _ptr(A.colidx), _ptr(A.vals),
-                                      _ptr(A.tasks) if plan else None, A.n_tasks if plan else 0, A.n_cta_tasks if plan else 0,
-                                      _ptr(A.split_rows) if plan else None, _ptr(A.counters) if plan else None,
-                                      _ptr(A.partial(d)) if plan else None,
-                                      _ptr(X), X.stride(0), _ptr(Y), d, _ptr(acc_in), _ptr(acc_out), d, float(acc_div),
-                                      _ptr(keep), float(scale), _stream()), "mmrec_spmm_drop_f32")
-        return
-    check(lib.mmrec_spmm_f32(A.n_rows, A.n_cols, d, _ptr(A.rowptr), _ptr(A.colidx), _ptr(A.vals),
-                             _ptr(A.tasks) if plan else None, A.n_tasks if plan else 0, A.n_cta_tasks if plan else 0,
-                             _ptr(A.split_rows) if plan else None, _ptr(A.counters) if plan else None,
-                             _ptr(A.partial(d)) if plan else None,
-                             _ptr(X), X.stride(0), _ptr(Y), d, _ptr(acc_in), _ptr(acc_out), d, float(acc_div),
-                             _ptr(gate_ref), d, _stream()), "mmrec_spmm_f32")
+    op = _spmm_op(A, X, Y=Y, acc_in=acc_in, acc_out=acc_out, acc_div=acc_div, gate_ref=gate_ref, y_accumulate=y_accumulate,
+                  drop=drop, use_plan=use_plan)
+    check(lib.mmrec_spmm_run_f32(d, 1, ctypes.byref(op), 0, _stream()), "mmrec_spmm_run_f32")
+
+
+def _spmm_op(A: CSR, X, Y=None, acc_in=None, acc_out=None, acc_div=1.0, gate_ref=None, y_accumulate=False, drop=None, post=None,
+             post_row0=0, sync_before=False, use_plan=True):
+    """One `mmrec_spmm_op` over A's work plan (none with `use_plan=False` or an empty plan).  X and acc_in are a tensor or a
+    (rows below the split, rows from the split on) pair; the other operands have leading dimension d."""
+    X_lo, X_hi = X if isinstance(X, tuple) else (X, None)
+    in_lo, in_hi = acc_in if isinstance(acc_in, tuple) else (acc_in, None)
+    d = X_lo.shape[1]
+    op = _lib.SpmmOp(n_rows=A.n_rows, n_cols=A.n_cols, rowptr=_ptr(A.rowptr), colidx=_ptr(A.colidx), vals=_ptr(A.vals),
+                     X=_ptr(X_lo), ldx=X_lo.stride(0), Y=_ptr(Y), ldy=d, y_accumulate=int(y_accumulate),
+                     acc_in=_ptr(in_lo), acc_out=_ptr(acc_out), ldacc=d, acc_div=float(acc_div), gate_ref=_ptr(gate_ref), ldgate=d,
+                     post=_ptr(post), ldpost=d, post_row0=int(post_row0), sync_before=int(bool(sync_before)))
+    if use_plan and A.n_tasks > 0:
+        op.tasks, op.n_tasks, op.n_cta_tasks = _ptr(A.tasks), A.n_tasks, A.n_cta_tasks
+        op.split_rows, op.counters, op.partial = _ptr(A.split_rows), _ptr(A.counters), _ptr(A.partial(d))
+    if X_hi is not None:
+        op.X_hi, op.ldx_hi, op.x_split = _ptr(X_hi), X_hi.stride(0), X_lo.shape[0]
+    if in_hi is not None:
+        op.acc_in_hi, op.ldacc_in_hi, op.acc_in_split = _ptr(in_hi), in_hi.stride(0), in_lo.shape[0]
+    if drop is not None:
+        op.keep_bits, op.keep_scale = _ptr(drop[0]), float(drop[1])
+    return op
 
 
 class _SpmmFn(torch.autograd.Function):
@@ -323,32 +328,9 @@ def spmm(A: CSR, X: torch.Tensor, base: Optional[torch.Tensor] = None) -> torch.
     return _SpmmFn.apply(X, A, base)
 
 
-def _chain_step(A: CSR, X, Y=None, acc_in=None, acc_out=None, acc_div=1.0, post=None, post_row0=0, sync_before=False):
-    """One `mmrec_spmm_step2`.  X and acc_in are a tensor or a (rows below the split, rows from the split on) pair."""
-    st2 = _lib.SpmmStep2()
-    st = st2.step
-    X_lo, X_hi = X if isinstance(X, tuple) else (X, None)
-    in_lo, in_hi = acc_in if isinstance(acc_in, tuple) else (acc_in, None)
-    d = X_lo.shape[1]
-    st.n_rows, st.n_cols = A.n_rows, A.n_cols
-    st.rowptr, st.colidx, st.vals = _ptr(A.rowptr), _ptr(A.colidx), _ptr(A.vals)
-    st.tasks, st.n_tasks, st.n_cta_tasks = _ptr(A.tasks), A.n_tasks, A.n_cta_tasks
-    st.split_rows, st.counters, st.partial = _ptr(A.split_rows), _ptr(A.counters), _ptr(A.partial(d))
-    st.X, st.ldx = _ptr(X_lo), X_lo.stride(0)
-    st.Y, st.ldy = _ptr(Y), d
-    st.acc_in, st.acc_out, st.ldacc, st.acc_div = _ptr(in_lo), _ptr(acc_out), d, float(acc_div)
-    st.post, st.ldpost, st.post_row0 = _ptr(post), d, int(post_row0)
-    st.sync_before = int(bool(sync_before))
-    if X_hi is not None:
-        st2.X_hi, st2.ldx_hi, st2.x_split = _ptr(X_hi), X_hi.stride(0), X_lo.shape[0]
-    if in_hi is not None:
-        st2.acc_in_hi, st2.ldacc_in_hi, st2.acc_in_split = _ptr(in_hi), in_hi.stride(0), in_lo.shape[0]
-    return st2
-
-
 def propagate_mean_fused(A: CSR, ego, n_layers: int, post_csr: Optional[CSR] = None, post_x: Optional[torch.Tensor] = None,
                          post_layers: int = 1, post_row0: int = 0, cooperative: bool = True) -> torch.Tensor:
-    """Inference form of `propagate_mean` (+ FREEDOM / BM3's item-item term) through `mmrec_spmm_steps_f32`:
+    """Inference form of `propagate_mean` (+ FREEDOM / BM3's item-item term) as one `mmrec_spmm_run_f32` call:
     `mean(E_0 .. E_L)`, and if `post_csr` is given `out[post_row0:] += post_csr^post_layers @ post_x`
     (`src/models/freedom.py:164-178`: `h = mm_adj @ ... @ item_emb`, `i_g + h`).  No autograd.
 
@@ -357,7 +339,6 @@ def propagate_mean_fused(A: CSR, ego, n_layers: int, post_csr: Optional[CSR] = N
     `cooperative`: all steps in one cooperative launch with grid barriers; otherwise one ordinary launch per group of
     independent steps (the item-item product shares layer 1's launch, each later layer is one launch).  Falls back to one
     launch per SpMM when the chained kernel does not take the shape."""
-    import ctypes
     pair = isinstance(ego, (tuple, list))
     parts = [_f32c(t) for t in ego] if pair else [_f32c(ego)]
     _need_cuda(*parts, post_x)
@@ -398,12 +379,12 @@ def propagate_mean_fused(A: CSR, ego, n_layers: int, post_csr: Optional[CSR] = N
     if len(waves) > 8:
         return unfused()
     waves.sort(key=lambda w: (w[0], w[1]))                          # within a wave: the A_hat layer first, the shorter product fills its tail
-    steps = [_chain_step(M, sync_before=i > 0 and w != waves[i - 1][0], **kw) for i, (w, _, M, kw) in enumerate(waves)]
-    arr = (_lib.SpmmStep2 * len(steps))(*steps)
-    rc = _lib.load().mmrec_spmm_steps_f32(d, len(steps), ctypes.cast(arr, ctypes.c_void_p), int(cooperative), _stream())
+    arr = (_lib.SpmmOp * len(waves))(*[_spmm_op(M, sync_before=i > 0 and w != waves[i - 1][0], **kw)
+                                         for i, (w, _, M, kw) in enumerate(waves)])
+    rc = _lib.load().mmrec_spmm_run_f32(d, len(arr), arr, int(cooperative), _stream())
     if rc == -4:                                                     # MMREC_EUNSUPPORTED: shape without a chained kernel
         return unfused()
-    check(rc, "mmrec_spmm_steps_f32")
+    check(rc, "mmrec_spmm_run_f32")
     return acc
 
 
@@ -499,7 +480,7 @@ def propagate_mean_dropped(A: CSR, ego: torch.Tensor, n_layers: int, keep: torch
                            scale: float) -> torch.Tensor:
     """`propagate_mean` through the edge-dropped matrix of SelfCF's encoder (`src/common/encoders.py:90-112`: `sparse_dropout`
     of the normalised adjacency, then `torch.sparse.mm` per layer and the layer mean), on the fixed CSR and its fixed plan:
-    the entries whose bit of `keep` is set, weighted fl(v * scale) (`mmrec_spmm_drop_f32`).  Differentiable w.r.t. `ego`; the
+    the entries whose bit of `keep` is set, weighted fl(v * scale) (`mmrec_spmm_op.keep_bits`).  Differentiable w.r.t. `ego`; the
     backward runs the same CSR with `keep_t` (`edge_keep_bits` with the mirror map), as A is symmetric bit for bit."""
     if not A.symmetric:
         raise MMRecError("propagate_mean_dropped: the backward reads the transpose through the mirrored bits; A must be symmetric")

@@ -25,20 +25,30 @@ def test_library_built_and_exports_every_header_symbol():
     assert set(names) == set(_lib.PROTOTYPES), "python prototypes and header disagree"
 
 
-def test_loader_binds_and_reports_version():
+def test_loader_binds_and_reports_abi_version():
     from mmrec_b200 import _lib
     lib = _lib.load()
-    assert lib.mmrec_abi_version() == _lib.ABI_VERSION == 3
+    assert lib.mmrec_abi_version() == _lib.ABI_VERSION == 4
     assert lib.mmrec_last_error() is not None
 
 
-def test_argument_errors_without_a_gpu():
+def test_argument_errors_before_any_cuda_call():
     """Argument validation happens before any CUDA call, so it is testable on a CPU box."""
     from mmrec_b200 import _lib
     lib = _lib.load()
-    assert lib.mmrec_spmm_f32(-1, 0, 64, None, None, None, None, 0, 0, None, None, None, None, 0, None, 0, None, None, 0,
-                              1.0, None, 0, None) == -1
+    op = _lib.SpmmOp(n_rows=-1, ldx=64, ldy=64, ldacc=64, acc_div=1.0)
+    assert lib.mmrec_spmm_run_f32(64, 1, ctypes.byref(op), 0, None) == -1
     assert b"spmm" in lib.mmrec_last_error()
+    assert lib.mmrec_spmm_run_f32(64, 0, ctypes.byref(op), 0, None) == -1                  # no ops
+    assert lib.mmrec_spmm_run_f32(64, 1, None, 0, None) == -1
+    # well-formed ops on fake, 16-byte aligned addresses with a work plan: rejected before any CUDA call
+    fake = dict(n_rows=8, n_cols=8, rowptr=0x1000, colidx=0x2000, vals=0x3000, tasks=0x4000, n_tasks=8, n_cta_tasks=0,
+                split_rows=0x5000, counters=0x6000, partial=0x7000, Y=0x8000, ldy=48, acc_div=1.0)
+    op = _lib.SpmmOp(X=0x9000, ldx=48, keep_bits=0xa000, keep_scale=1.0, **fake)
+    assert lib.mmrec_spmm_run_f32(48, 1, ctypes.byref(op), 0, None) == -4                 # edge-keep mask at d = 48
+    ops = (_lib.SpmmOp * 2)(_lib.SpmmOp(X=0x9000, ldx=64, **dict(fake, ldy=64)),
+                            _lib.SpmmOp(X=0x9000, ldx=64, gate_ref=0xa000, ldgate=64, **dict(fake, ldy=64)))
+    assert lib.mmrec_spmm_run_f32(64, 2, ops, 0, None) == -4                               # the chained kernel has no gate
     assert lib.mmrec_topk_rows_f32(4, 10, None, 10, 11, 0, None, None, None) == -1     # k > n_items
     assert lib.mmrec_project_f32(-5, None, None, 0, 0, None, None, 0, 0, None, 0, None, 0, None) == -1
     assert lib.mmrec_topk_merge(100, 4, 50, None, None, None, None, None) == -1        # parts * k > 4096

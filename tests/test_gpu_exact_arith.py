@@ -132,7 +132,7 @@ def _run_epilogues(dev, case, use_plan, what):
     wy, wa = O.spmm_epilogue_f32(case.y, case.acc_in, 1.0, gate_ref=case.ref)
     O.assert_bits(Yg, wy, f"{what} gated Y")
     O.assert_bits(accg, wa, f"{what} gated acc_out")
-    # Y += A X (mmrec_spmm_acc_f32) with a running sum
+    # Y += A X (y_accumulate) with a running sum
     Ya = torch.from_numpy(case.acc_in).to(dev).clone()
     outa = torch.empty(n, d, device=dev)
     ops.spmm_raw(case.A, case.X, Y=Ya, acc_in=acc_in, acc_out=outa, acc_div=3.0, use_plan=use_plan, y_accumulate=True)
@@ -170,17 +170,18 @@ def test_spmm_generic_widths(dev, d):
 
 
 def _spmm_abi(case, d, X, ldx, Y, ldy, acc_in, acc_out, ldacc, acc_div, ref, ldref):
-    """`mmrec_spmm_f32` with raw addresses and leading dimensions (ops.spmm_raw would copy to contiguous operands)."""
+    """`mmrec_spmm_run_f32` with raw addresses and leading dimensions (ops.spmm_raw would copy to contiguous operands)."""
     from mmrec_b200 import _lib
     A = case.A
-    _lib.check(_lib.load().mmrec_spmm_f32(A.n_rows, A.n_cols, d, A.rowptr.data_ptr(), A.colidx.data_ptr(), A.vals.data_ptr(),
-                                          A.tasks.data_ptr(), A.n_tasks, A.n_cta_tasks, A.split_rows.data_ptr(), A.counters.data_ptr(),
-                                          A.partial(d).data_ptr(), X, ldx, Y, ldy, acc_in, acc_out, ldacc, acc_div, ref, ldref,
-                                          torch.cuda.current_stream().cuda_stream), "mmrec_spmm_f32")
+    op = _lib.SpmmOp(n_rows=A.n_rows, n_cols=A.n_cols, rowptr=A.rowptr.data_ptr(), colidx=A.colidx.data_ptr(), vals=A.vals.data_ptr(),
+                     tasks=A.tasks.data_ptr(), n_tasks=A.n_tasks, n_cta_tasks=A.n_cta_tasks, split_rows=A.split_rows.data_ptr(),
+                     counters=A.counters.data_ptr(), partial=A.partial(d).data_ptr(), X=X, ldx=ldx, Y=Y, ldy=ldy,
+                     acc_in=acc_in, acc_out=acc_out, ldacc=ldacc, acc_div=acc_div, gate_ref=ref, ldgate=ldref)
+    _lib.check(_lib.load().mmrec_spmm_run_f32(d, 1, ctypes.byref(op), 0, torch.cuda.current_stream().cuda_stream), "mmrec_spmm_run_f32")
 
 
 @pytest.mark.parametrize("d,shift", [(64, 1), (128, 2), (32, 0)])
-def test_spmm_misaligned_and_strided_through_the_c_abi(dev, d, shift):
+def test_spmm_misaligned_and_strided_through_the_op_descriptor(dev, d, shift):
     """Misaligned X / Y / acc (offset by `shift` floats) and leading dimensions > d reach the generic kernel; shift 0
     with padded rows (ld % 4 == 0, 16-byte aligned) keeps the vector kernel on strided operands."""
     case = _SpmmCase(dev, d)
@@ -221,8 +222,8 @@ def test_spmm_transpose(dev, d):
 
 @pytest.mark.parametrize("d", [64, 128])
 def test_spmm_panel_csr(dev, d):
-    """`mmrec_spmm_acc_f32` through PanelCSR: Y and the running sum accumulate over ~5 column panels; the division comes
-    with the last one."""
+    """The accumulating Y (y_accumulate) through PanelCSR: Y and the running sum accumulate over ~5 column panels; the
+    division comes with the last one."""
     from mmrec_b200 import ops
     case = _SpmmCase(dev, d)
     r, c, v = case.A.coo()

@@ -1,12 +1,11 @@
 """Inference propagation straight from the embedding tables.
 
 `ops.propagate_mean_fused` takes E_0 as the pair (user table, item table): layer 1 gathers from the two tables and adds
-them to the running sum where they are (`mmrec_spmm_steps_f32`'s two-block X / acc_in), the item-item product shares layer
+them to the running sum where they are (`mmrec_spmm_op`'s two-block X / acc_in), the item-item product shares layer
 1's launch, later layers are one ordinary launch each.  FREEDOM, BM3 and MGCN run it in inference; their outputs must be
 the bits of the route it replaces: concatenate the tables, one SpMM launch per layer, then the item-item product with the
 layer mean as its base.
 """
-import ctypes
 
 import numpy as np
 import pytest
@@ -85,8 +84,8 @@ def _two_block(t, split, ld_hi):
 
 @pytest.mark.parametrize("cooperative", [0, 1])
 @pytest.mark.parametrize("d", [32, 64, 256])
-def test_steps_two_block_operands_bit_for_bit(dev, d, cooperative):
-    """mmrec_spmm_steps_f32 with X and acc_in in two row blocks (own splits, the second block strided) against the exact
+def test_run_two_block_operands_bit_for_bit(dev, d, cooperative):
+    """mmrec_spmm_run_f32 with X and acc_in in two row blocks (own splits, the second block strided) against the exact
     result and against the same steps on the concatenated operands: a square matrix with split rows (513, 520, 4200
     non-zeros) and CTA-sized rows, splits that fall inside both, an independent product sharing the launch, the mean and
     `+ post` on the last rows."""
@@ -121,12 +120,10 @@ def test_steps_two_block_operands_bit_for_bit(dev, d, cooperative):
 
     def run(Xop, Iop):
         Y, acc, hm = torch.empty(n, d, device=dev), torch.empty(n, d, device=dev), torch.empty(n_post, d, device=dev)
-        steps = [ops._chain_step(A, Xop, Y=Y, acc_in=Iop, acc_out=acc, acc_div=3.0, post=post_t, post_row0=row0),
-                 ops._chain_step(M, x_post, Y=hm)]
-        arr = (_lib.SpmmStep2 * 2)(*steps)
+        arr = (_lib.SpmmOp * 2)(ops._spmm_op(A, Xop, Y=Y, acc_in=Iop, acc_out=acc, acc_div=3.0, post=post_t, post_row0=row0),
+                                ops._spmm_op(M, x_post, Y=hm))
         before = ops.launch_count()
-        _lib.check(lib.mmrec_spmm_steps_f32(d, 2, ctypes.cast(arr, ctypes.c_void_p), cooperative, torch.cuda.current_stream().cuda_stream),
-                   "mmrec_spmm_steps_f32")
+        _lib.check(lib.mmrec_spmm_run_f32(d, 2, arr, cooperative, torch.cuda.current_stream().cuda_stream), "mmrec_spmm_run_f32")
         assert ops.launch_count() - before == 1
         return Y, acc, hm
 

@@ -463,7 +463,7 @@ def test_spmm_two_streams(sq, d):
 
 
 def test_spmm_drop_two_streams(sq):
-    """The edge-dropout kernel (`mmrec_spmm_drop_f32`) with different keep bits and X per stream."""
+    """The edge-dropout kernel (`mmrec_spmm_op.keep_bits`) with different keep bits and X per stream."""
     from mmrec_b200 import ops
     A, Ai = sq
     rng = np.random.default_rng(11)

@@ -672,8 +672,8 @@ def test_evaluator_routes_to_the_host(dev, monkeypatch, route):
 
 @pytest.mark.parametrize("d,L,mm_layers", [(64, 3, 1), (64, 1, 1), (128, 2, 2), (32, 4, 0), (64, 2, 0)])
 def test_spmm_chain_equals_separate_launches(dev, d, L, mm_layers):
-    """mmrec_spmm_chain_f32 (all SpMMs of a propagation in one cooperative launch, grid barriers in between) runs the same
-    kernel body as mmrec_spmm_f32: bit-identical to the one-launch-per-SpMM path, also when replayed from a CUDA graph."""
+    """The cooperative form of mmrec_spmm_run_f32 (all SpMMs of a propagation in one launch, grid barriers in between) runs
+    the same kernel body as a single product: bit-identical to the one-launch-per-SpMM path, also when replayed from a CUDA graph."""
     from mmrec_b200 import ops
     from mmrec_b200.ops import CSR
     U, I = 900, 500

@@ -1,4 +1,4 @@
-"""SELFCFED_LGN's edge dropout inside K1 (`mmrec_spmm_drop_f32`, `mmrec_edge_keep_bits`) and the model class.
+"""SELFCFED_LGN's edge dropout inside K1 (`mmrec_spmm_op.keep_bits`, `mmrec_edge_keep_bits`) and the model class.
 
 The masked SpMM is checked bit for bit against the unmasked kernel on the compacted matrix (the kept entries, values
 fl(v * scale)) on exactly representable operands (integers times a power of two, every partial sum exact: see
