@@ -476,6 +476,39 @@ int mmrec_mgcn_fuse_f32(int64_t n, int d, const float* img, const float* txt, co
                         const float* wq2, const float* Wgi, const float* bgi, const float* Wgt, const float* bgt, float* out,
                         float* side, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * n9  MMGCF's late fusion, element-wise modes.   Replaces `fuse_item_embeddings` (src/models/mmgcf.py:177-254: the
+ * `F.normalize` / `* alpha` / `* (1 - alpha)` scalings, `_apply_fusion`'s `torch.stack(...).mean(0)` / `.sum(0)`, and
+ * equal's two stages) on the rows `calculate_loss` reads (`ia_emb[pos_items]`, `ia_emb[neg_items]`, :270-284), and its
+ * autograd; the `ia_emb[...]` gathers and their backward scatter go with it.
+ *   out[r,:] = combine(c_e n(E[idx ? idx[r] : r, :]), c_m n(V[r,:]), c_m n(T[r,:]))          r < n
+ *   fusion     0 mean (`stack(..).mean(0)`), 1 sum (`.sum(0)`)
+ *   weighting  0 equal: combine(E row, combine(V, T)), n = identity, c = 1 (one modality: combine(E row, V or T));
+ *              1 alpha: c_e = alpha[0], c_m = 1 - alpha[0], n = identity (alpha: ONE fp32 on the device, sigmoid(mm_alpha));
+ *              2 normalized: n(x) = x / max(||x||_2, 1e-12), c_e = number of modalities, c_m = 1
+ *   E [n_E, d] (the propagated item rows), V / T [n, d] (the projected modality rows of the same items; either may be
+ *   NULL, not both), out [n, d]; every matrix row-major with leading dimension d.  idx int64 [n], may repeat and need not
+ *   be sorted; entries must lie in [0, n_E) (not checked).  idx == NULL reads row r of E (n <= n_E).
+ *   Rounding: every torch step is one IEEE fp32 rounding in torch's order; a mean of k terms is the sum times fl(1/k), as
+ *   ATen's CUDA reduction does, and its backward multiplies by fl(1/k), as autograd's `grad / k` runs on the device.  With
+ *   equal and alpha the results equal the torch expression on the device bit for bit; with normalized the row norms are
+ *   the kernel's own reduction (held to a bound, tests/test_gpu_mmgcf.py).
+ * mmrec_late_fuse_bwd_f32: for the upstream gradient g [n, d]: dE_rows [n, d] (row r belongs to E row idx[r]: scatter it
+ *   with mmrec_index_sum_rows_f32), dV / dT [n, d] (required for the modalities given), and under alpha *dalpha (one fp32
+ *   on the device) = sum over the rows of <g', E row> - <g', V row> - <g', T row> (g' = g after the mean's factor): per-CTA
+ *   partials in ws, summed by one warp in a fixed order, bit-reproducible.  Norms are recomputed, nothing is stored by the
+ *   forward.  ws from mmrec_late_fuse_workspace_bytes(n, d), read only under alpha.
+ * Both: d in {32, 64, 128} (else MMREC_EUNSUPPORTED), one warp per row; a bad mode, size or null pointer returns
+ * MMREC_EINVAL and a small workspace MMREC_EWORKSPACE, before any CUDA call.  n == 0 returns at once (the backward sets
+ * *dalpha = 0).
+ * ------------------------------------------------------------------------------------------- */
+size_t mmrec_late_fuse_workspace_bytes(int64_t n, int d);
+int mmrec_late_fuse_f32(int64_t n, int d, int fusion, int weighting, const int64_t* idx, const float* E, int64_t n_E,
+                        const float* V, const float* T, const float* alpha, float* out, void* stream);
+int mmrec_late_fuse_bwd_f32(int64_t n, int d, int fusion, int weighting, const int64_t* idx, const float* E, int64_t n_E,
+                            const float* V, const float* T, const float* alpha, const float* g, float* dE_rows, float* dV,
+                            float* dT, float* dalpha, void* ws, size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -76,6 +76,9 @@ PROTOTYPES = {
     "mmrec_adam_f32": (_i32, [_i32, _p, _f64, _f64, _f64, _f64, _p]),
     "mmrec_gate_rows_f32": (_i32, [_i64, _i32, _p, _p, _p, _p, _p, _p]),
     "mmrec_mgcn_fuse_f32": (_i32, [_i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "mmrec_late_fuse_workspace_bytes": (_sz, [_i64, _i32]),
+    "mmrec_late_fuse_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _i64, _p, _p, _p, _p, _p]),
+    "mmrec_late_fuse_bwd_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
 }
 
 class SpmmOp(C.Structure):

@@ -691,6 +691,84 @@ def mgcn_fuse(img, txt, content, q_w, q_b, q_w2, gi_w, gi_b, gt_w, gt_b, want_si
     return (out, side) if want_side else out
 
 
+# -- n9: MMGCF's late fusion (csrc/fuse.cu) ---------------------------------------------------------------------------
+LATE_FUSIONS = ("mean", "sum")
+LATE_WEIGHTINGS = ("equal", "alpha", "normalized")
+
+
+def _late_fuse_args(item_e, mods, idx, fusion, weighting, alpha):
+    """Validated, contiguous operands of `mmrec_late_fuse_*` -- every check before anything reaches the device."""
+    if fusion not in LATE_FUSIONS:
+        raise MMRecError(f"late_fuse: fusion {fusion!r} is not one of {LATE_FUSIONS}")
+    if weighting not in LATE_WEIGHTINGS:
+        raise MMRecError(f"late_fuse: weighting {weighting!r} is not one of {LATE_WEIGHTINGS}")
+    mods = [m for m in mods if m is not None]
+    if not 1 <= len(mods) <= 2:
+        raise MMRecError(f"late_fuse: one or two modality tables, got {len(mods)}")
+    if (alpha is not None) != (weighting == "alpha"):
+        raise MMRecError("late_fuse: alpha is given exactly when weighting is 'alpha'")
+    if item_e.dim() != 2 or any(m.dim() != 2 for m in mods):
+        raise MMRecError("late_fuse: item_e and the modality tables must be 2-D")
+    d = item_e.shape[1]
+    if d not in (32, 64, 128):
+        raise MMRecError(f"late_fuse: d = {d} has no kernel (32, 64, 128)")
+    n = item_e.shape[0] if idx is None else idx.numel()
+    for m in mods:
+        if tuple(m.shape) != (n, d):
+            raise MMRecError(f"late_fuse: modality rows must be [{n}, {d}], got {tuple(m.shape)}")
+    if alpha is not None and alpha.numel() != 1:
+        raise MMRecError("late_fuse: alpha must hold one element")
+    _need_cuda(item_e, *mods, idx, alpha)
+    idx = None if idx is None else idx.to(torch.int64).contiguous()
+    alpha = None if alpha is None else _f32c(alpha.reshape(1))
+    return _f32c(item_e), [_f32c(m) for m in mods], idx, n, d, LATE_FUSIONS.index(fusion), LATE_WEIGHTINGS.index(weighting), alpha
+
+
+class _LateFuseFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, item_e, v, t, alpha, idx, fusion: int, weighting: int):
+        n, d = (item_e.shape[0] if idx is None else idx.numel()), item_e.shape[1]
+        out = torch.empty(n, d, dtype=torch.float32, device=item_e.device)
+        check(_lib.load().mmrec_late_fuse_f32(n, d, fusion, weighting, _ptr(idx), _ptr(item_e), item_e.shape[0], _ptr(v), _ptr(t),
+                                              _ptr(alpha), _ptr(out), _stream()), "mmrec_late_fuse_f32")
+        ctx.save_for_backward(item_e, v, t, alpha, idx)
+        ctx.modes = (fusion, weighting)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        item_e, v, t, alpha, idx = ctx.saved_tensors
+        fusion, weighting = ctx.modes
+        lib = _lib.load()
+        g = _f32c(g)
+        n, d = g.shape
+        dE = torch.empty(n, d, dtype=torch.float32, device=g.device)
+        dv = None if v is None else torch.empty_like(dE)
+        dt = None if t is None else torch.empty_like(dE)
+        da = None if alpha is None else torch.empty(1, dtype=torch.float32, device=g.device)
+        ws = _ws("late_fuse", lib.mmrec_late_fuse_workspace_bytes(n, d), g.device)
+        check(lib.mmrec_late_fuse_bwd_f32(n, d, fusion, weighting, _ptr(idx), _ptr(item_e), item_e.shape[0], _ptr(v), _ptr(t),
+                                          _ptr(alpha), _ptr(g), _ptr(dE), _ptr(dv), _ptr(dt), _ptr(da), _ptr(ws), ws.numel(),
+                                          _stream()), "mmrec_late_fuse_bwd_f32")
+        if idx is not None and ctx.needs_input_grad[0]:
+            dE = index_sum_rows(dE, idx, item_e.shape[0])             # ascending j: bit-reproducible, unlike index_add_
+        return dE, dv, dt, da, None, None, None
+
+
+def late_fuse(item_e: torch.Tensor, v: Optional[torch.Tensor], t: Optional[torch.Tensor], fusion: str, weighting: str,
+              alpha: Optional[torch.Tensor] = None, idx: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """MMGCF's element-wise late fusion (`src/models/mmgcf.py:177-254`, `fusion_mode` mean | sum x `weighting`
+    equal | alpha | normalized) of the item rows `item_e[idx]` (all rows when idx is None) with the projected modality rows
+    `v` / `t` of the same items (either may be None), in one kernel (`mmrec_late_fuse_f32`), differentiable w.r.t.
+    item_e, v, t and alpha.  `alpha` is `sigmoid(mm_alpha)` as a one-element device tensor (weighting 'alpha' only): it
+    is read on the device, so the call never synchronises.  The gradient of item_e is the per-row gradient scattered by
+    `index_sum_rows`.  With 'equal' and 'alpha' the values equal the torch expression on the device bit for bit, forward
+    and backward (d alpha: to fp32 reorder error, the same bits on every run); 'normalized' is held to a bound."""
+    item_e, mods, idx, n, d, fu, we, alpha = _late_fuse_args(item_e, (v, t), idx, fusion, weighting, alpha)
+    v, t = (mods[0], mods[1]) if len(mods) == 2 else ((mods[0], None) if v is not None else (None, mods[0]))
+    return _LateFuseFn.apply(item_e, v, t, alpha, idx, fu, we)
+
+
 # ------------------------------------------------------------------------------------------------
 # K3: scoring, mask, top-k
 # ------------------------------------------------------------------------------------------------
