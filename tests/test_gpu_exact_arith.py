@@ -163,10 +163,18 @@ def test_spmm_vec_every_lane_width_and_epilogue(dev, d, lanes, use_plan):
         lib.mmrec_spmm_set_lanes(0)
 
 
-@pytest.mark.parametrize("d", [5, 48, 96])
+@pytest.mark.parametrize("d", [5, 48, 100])
 def test_spmm_generic_widths(dev, d):
     """Widths without a vector instance run the generic kernel (whole rows, scalar loads)."""
     _run_epilogues(dev, _SpmmCase(dev, d), True, f"generic d={d}")
+
+
+@pytest.mark.parametrize("use_plan", [True, False])
+@pytest.mark.parametrize("d", [96, 192, 384])
+def test_spmm_vec_3d_every_epilogue(dev, d, use_plan):
+    """The width-3d instances (three float4 per lane, SLMRec's three views side by side), every epilogue: the gate and
+    Y += A X included, which reduce or read across the whole 3d row."""
+    _run_epilogues(dev, _SpmmCase(dev, d), use_plan, f"3d d={d} plan={use_plan}")
 
 
 def _spmm_abi(case, d, X, ldx, Y, ldy, acc_in, acc_out, ldacc, acc_div, ref, ldref):
