@@ -275,8 +275,10 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
     const int64_t n_heavy = p.tasks ? p.n_heavy : 0;
 
     // ---------------- phase 1: CTA-cooperative tasks
+    int4 tk_next = (int64_t)blockIdx.x < n_heavy ? __ldg(p.tasks + blockIdx.x) : make_int4(0, 0, 0, -1);
     for (int64_t ct = blockIdx.x; ct < n_heavy; ct += gridDim.x) {
-        const int4 tk = __ldg(p.tasks + ct);
+        const int4 tk = tk_next;
+        if (ct + gridDim.x < n_heavy) tk_next = __ldg(p.tasks + ct + gridDim.x);   // in flight during this task
         const int row = tk.x, sid = tk.w;
         const int len = tk.z - tk.y;
         const int chunk = (len + G - 1) / G;
@@ -359,8 +361,12 @@ __device__ __forceinline__ void spmm_vec_body(const SpmmParams& p, float* __rest
     }
 }
 
+// One float4 per lane (V = 1, every default width d <= 128): capped at 64 registers, so 4 CTAs (32 warps) per SM instead of
+// the 3 that 74 registers allow at d = 32 / 64 -- the kernel is bound by dependent-load latency, and a third more warps in
+// flight per SM is a third more rows of X in flight; no spills (DESIGN.md section 4, K1).  Other widths keep the compiler's
+// choice (minimum blocks 0 = unspecified): forcing 4 CTAs there spills.
 template <int D, int T>
-__global__ void __launch_bounds__(256) spmm_vec_kernel(const SpmmParams p) {
+__global__ void __launch_bounds__(256, VecCfg<D, T>::V == 1 ? 4 : 0) spmm_vec_kernel(const SpmmParams p) {
     __shared__ __align__(16) float red[(256 / T) * D];
     spmm_vec_body<D, T, false>(p, red);
 }
