@@ -509,6 +509,24 @@ int mmrec_late_fuse_bwd_f32(int64_t n, int d, int fusion, int weighting, const i
                             const float* V, const float* T, const float* alpha, const float* g, float* dE_rows, float* dV,
                             float* dT, float* dalpha, void* ws, size_t ws_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * n11  SDDMM: the values gradient of a CSR product.   Replaces the dense [I, I] gradient of
+ * `torch.mm(item_adj, h)` w.r.t. LATTICE's learned item graph (src/models/lattice.py:162-163) and the dense cosine
+ * similarities `build_sim` forms only to keep knn_k of them per row (src/utils/utils.py:119-137).
+ *   out[e] = <P[row(e), :], Q[colidx[e], :]>   for every stored entry e of the n_rows x n_cols CSR (rowptr, colidx)
+ *   P [n_rows, d] (leading dimension ldp), Q [n_cols, d] (ldq), out fp32[nnz] in CSR order.  With P = dY and Q = X it is
+ *   dS of Y = S X on S's pattern.
+ *  - Every dot product runs in a fixed order that depends on d only (a group of 8 / 16 / 32 lanes for d <= 32 / <= 64 /
+ *    above: lane j sums k = j, j + group, ... with fmaf, then a fixed xor butterfly), so the bits are the same on every
+ *    run.  Any d >= 1; empty rows are allowed; NaN / inf propagate.  Column indices must lie in [0, n_cols) (not checked).
+ *  - Bad sizes (d < 1, ld < d, nnz > 0 in an empty matrix) or a null pointer return MMREC_EINVAL before any CUDA call;
+ *    nnz == 0 returns at once.
+ * The symmetric normalisation D^-1/2 A D^-1/2 of a CSR and its backward need no entry point of their own: their row and
+ * column reductions are width-1 products of mmrec_spmm_run_f32 (the generic kernel, rows in ascending stored order).
+ * ------------------------------------------------------------------------------------------- */
+int mmrec_sddmm_f32(int64_t n_rows, int64_t n_cols, int64_t nnz, const int32_t* rowptr, const int32_t* colidx,
+                    const float* P, int64_t ldp, const float* Q, int64_t ldq, int d, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

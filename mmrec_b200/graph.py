@@ -7,7 +7,10 @@ Reference code replaced (paths relative to the root of enoche/MMRec):
   * `MGCN.get_adj_mat`  -- src/models/mgcn.py:109-144 (lil-matrix slicing, 128 s at clothing scale);
   * `pre_epoch_processing` / `_normalize_adj_m` / `get_edge_info` -- src/models/freedom.py:128-162;
   * `get_knn_adj_mat` -- src/models/freedom.py:79-100 and `build_knn_normalized_graph` -- src/utils/utils.py:165-183
-    (init-time item-item graphs; SURVEY.md 8f f4: contraction and selection on the scoring kernels, `_knn`).
+    (init-time item-item graphs; SURVEY.md 8f f4: contraction and selection on the scoring kernels, `_knn`);
+  * `get_adj_mat` -- src/models/lattice.py:100-122 (LATTICE's D^-1 (A + I) through dok / lil): `lattice_norm_adj_entries`;
+  * `build_sim` / `build_knn_neighbourhood` / `compute_normalized_laplacian` -- src/utils/utils.py:119-137 (LATTICE's
+    dense [I, I] graphs): `build_mgcn_knn_adj` at construction, `knn_normalized` for the learned graph.
 """
 from __future__ import annotations
 
@@ -112,6 +115,38 @@ def build_slmrec_adj(inter, n_users, n_items, device, adj_type) -> CSR:
     n = n_users + n_items
     return CSR.from_coo(_to_dev(rows, device), _to_dev(cols, device), _to_dev(vals, device), n, n,
                         sum_duplicates=False, symmetric=adj_type in SLMREC_SYMMETRIC_ADJ)
+
+
+def lattice_norm_adj_entries(inter_row, inter_col, n_users, n_items):
+    """(rows, cols, vals fp32) of LATTICE's `get_adj_mat` (`src/models/lattice.py:100-122`): D^-1 (A + I), row-normalised
+    with self-loops.  The reference assigns R into a lil matrix, so a repeated (user, item) pair keeps its multiplicity m
+    as the entry's value (SLMRec's `nonzero()` makes it binary, `slmrec_adj_entries`); `sp.eye` is float64, so the row sums
+    and `np.power(rowsum, -1)` are float64 and each value is fl32(d_inv[r] * m), rounded once.  Entries in (row, col)
+    order; no dok or lil matrix is built."""
+    r = np.asarray(inter_row, dtype=np.int64)
+    c = np.asarray(inter_col, dtype=np.int64)
+    n = n_users + n_items
+    diag = np.arange(n, dtype=np.int64)
+    key = np.sort(np.concatenate([r * n + (c + n_users), (c + n_users) * n + r, diag * n + diag]), kind="stable")
+    start = np.empty(key.size, dtype=bool)
+    start[0] = True                                                   # n >= 1: the diagonal is never empty
+    np.not_equal(key[1:], key[:-1], out=start[1:])
+    first = np.flatnonzero(start)
+    mult = np.diff(np.append(first, key.size)).astype(np.float64)
+    ukey = key[first]
+    rows, cols = ukey // n, ukey % n
+    d_inv = np.power(np.bincount(rows, weights=mult, minlength=n), -1)
+    return rows, cols, (d_inv[rows] * mult).astype(np.float32)
+
+
+def build_lattice_norm_adj(inter, n_users, n_items, device) -> CSR:
+    """LATTICE's `norm_adj` as a device CSR, with its transpose (the backward's: the matrix is not symmetric)."""
+    r, c = (inter.row, inter.col) if hasattr(inter, "row") else inter
+    rows, cols, vals = lattice_norm_adj_entries(r, c, n_users, n_items)
+    n = n_users + n_items
+    A = CSR.from_coo(_to_dev(rows, device), _to_dev(cols, device), _to_dev(vals, device), n, n, sum_duplicates=False, symmetric=False)
+    A.t()
+    return A
 
 
 def dropout_entry_maps(inter_row, inter_col, n_users, n_items):
@@ -302,7 +337,13 @@ def _knn(feat: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None):
     fused and every value an exact fp32 fmaf chain, bit-identical to the route below at these widths (where `ops.score`
     is the exact CUDA-core kernel) without writing the [n, n] similarities.  F <= 128: `ops.score` (3xTF32 tensor-core
     path) in row blocks bounded to 256 MiB of similarities, then `ops.mask_topk` (radix select)."""
-    cn = feat.div(torch.norm(feat, p=2, dim=-1, keepdim=True)).contiguous()
+    return knn_normalized(feat.div(torch.norm(feat, p=2, dim=-1, keepdim=True)).contiguous(), k, rows)
+
+
+def knn_normalized(cn: torch.Tensor, k: int, rows: Optional[torch.Tensor] = None):
+    """`_knn` of features already divided by their row norms: (values, indices) [n_rows, k] of `cn @ cn.T`, no [n, n]
+    tensor beyond the bounded score blocks.  LATTICE's learned graph selects on its own normalised projections."""
+    cn = cn.contiguous()
     if cn.shape[1] > 128:
         return ops.knn_topk(cn, k, rows)
     n = cn.shape[0]

@@ -7,6 +7,7 @@ sm_90 device, otherwise `MMRecError` is raised.
 """
 from __future__ import annotations
 
+import copy
 import ctypes
 from typing import Optional
 
@@ -84,6 +85,8 @@ class CSR:
         self.seg = SEG if seg is None else seg
         self.light_max = LIGHT_MAX if light_max is None else light_max
         self._t: Optional["CSR"] = None
+        self._owner: Optional["CSR"] = None             # the CSR whose pattern and plan this one shares (with_values)
+        self._tp = None                                 # (transpose pattern, permutation), see transpose_pattern
         self._split = {}                                # (device, stream) -> split-row counters and partials, see _split_scratch
         self._plan()
 
@@ -182,6 +185,32 @@ class CSR:
             self._t = CSR.from_coo(c, r, v, self.n_cols, self.n_rows, False, False, self.seg, self.light_max)
             self._t._t = self
         return self._t
+
+    def with_values(self, vals: torch.Tensor) -> "CSR":
+        """This pattern, work plan and split-row scratch with other values `vals` (fp32 [nnz], CSR order): no sort, no plan.
+        Each epoch's learned item graph of LATTICE is one pattern whose values change with every autograd step."""
+        _need_cuda(vals)
+        vals = _f32c(vals)
+        if vals.dim() != 1 or vals.numel() != self.nnz:
+            raise MMRecError(f"CSR.with_values: expected {self.nnz} values, got shape {tuple(vals.shape)}")
+        out = copy.copy(self)
+        out.vals = vals if self.nnz else torch.zeros(1, dtype=torch.float32, device=vals.device)
+        out._owner, out._t, out._tp = self._owner or self, None, None
+        return out
+
+    def transpose_pattern(self):
+        """(T, perm): the transposed pattern with its own work plan, and int64 perm [nnz] such that the transpose of this
+        pattern with values v is `T.with_values(v[perm])`.  Built once per pattern and shared by every `with_values` copy."""
+        owner = self._owner or self
+        if owner._tp is None:
+            r, c, v = owner.coo()
+            perm = torch.argsort(c * max(owner.n_rows, 1) + r, stable=True)
+            rowptr = torch.zeros(owner.n_cols + 1, dtype=torch.int32, device=r.device)
+            rowptr[1:] = torch.cumsum(torch.bincount(c, minlength=owner.n_cols), 0).to(torch.int32)
+            colidx = r[perm].to(torch.int32) if owner.nnz else torch.zeros(1, dtype=torch.int32, device=r.device)
+            vt = v[perm].contiguous() if owner.nnz else torch.zeros(1, dtype=torch.float32, device=r.device)
+            owner._tp = (CSR(owner.n_cols, owner.n_rows, rowptr, colidx, vt, owner.nnz, False, owner.seg, owner.light_max), perm)
+        return owner._tp
 
     def to_dense(self) -> torch.Tensor:
         r, c, v = self.coo()
@@ -326,6 +355,140 @@ class _SpmmFn(torch.autograd.Function):
 def spmm(A: CSR, X: torch.Tensor, base: Optional[torch.Tensor] = None) -> torch.Tensor:
     """`base + A @ X` (base optional), differentiable w.r.t. X and base."""
     return _SpmmFn.apply(X, A, base)
+
+
+# -- n11: values gradients of CSR products (csrc/sddmm.cu) ---------------------------------------------------------------
+def sddmm_raw(A: CSR, P: torch.Tensor, Q: torch.Tensor) -> torch.Tensor:
+    """out[e] = <P[row(e)], Q[col(e)]> over A's stored entries, fp32 [nnz] in CSR order (`mmrec_sddmm_f32`, no autograd).
+    Each dot product runs in a fixed order, so the bits are the same on every run."""
+    _need_cuda(P, Q)
+    if P.dim() != 2 or Q.dim() != 2 or P.shape[0] != A.n_rows or Q.shape[0] != A.n_cols or P.shape[1] != Q.shape[1] or P.shape[1] < 1:
+        raise MMRecError(f"sddmm: P [{A.n_rows}, d] and Q [{A.n_cols}, d] with d >= 1 expected, got {tuple(P.shape)} and {tuple(Q.shape)}")
+    P, Q = _f32c(P), _f32c(Q)
+    out = torch.empty(max(A.nnz, 1), dtype=torch.float32, device=P.device)[:A.nnz]
+    check(_lib.load().mmrec_sddmm_f32(A.n_rows, A.n_cols, A.nnz, _ptr(A.rowptr), _ptr(A.colidx), _ptr(P), P.stride(0), _ptr(Q),
+                                      Q.stride(0), P.shape[1], _ptr(out), _stream()), "mmrec_sddmm_f32")
+    return out
+
+
+def _spmm_new(A: CSR, X: torch.Tensor, base: Optional[torch.Tensor] = None) -> torch.Tensor:
+    out = torch.empty(A.n_rows, X.shape[1], dtype=torch.float32, device=X.device)
+    if base is None:
+        spmm_raw(A, X, Y=out)
+    else:
+        spmm_raw(A, X, acc_in=base, acc_out=out)
+    return out
+
+
+def _spmm_both(A: CSR, s: torch.Tensor, X: torch.Tensor) -> torch.Tensor:
+    """S X + S^T X for the square pattern A with values s: two K1 products, the second adding the first in its epilogue."""
+    T, perm = A.transpose_pattern()
+    return _spmm_new(T.with_values(s[perm]), X, base=_spmm_new(A.with_values(s), X))
+
+
+class _SddmmFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, P, Q, A: CSR):
+        ctx.A = A
+        ctx.save_for_backward(P, Q)
+        return sddmm_raw(A, P, Q)
+
+    @staticmethod
+    def backward(ctx, g):
+        P, Q = ctx.saved_tensors
+        A, g = ctx.A, _f32c(g)
+        dP = dQ = None
+        if ctx.needs_input_grad[0]:
+            dP = _spmm_new(A.with_values(g), Q)                        # dP = S Q, S = A's pattern with the value gradients
+        if ctx.needs_input_grad[1]:
+            T, perm = A.transpose_pattern()
+            dQ = _spmm_new(T.with_values(g[perm]), P)                 # dQ = S^T P
+        return dP, dQ, None
+
+
+def sddmm(A: CSR, P: torch.Tensor, Q: torch.Tensor) -> torch.Tensor:
+    """`sddmm_raw`, differentiable w.r.t. P and Q: dP = S Q and dQ = S^T P with S = A's pattern carrying the upstream
+    gradient, two K1 products.  With P = Q = the row-normalised features it is the cosine of the selected pairs of
+    `build_sim` + `build_knn_neighbourhood` (src/utils/utils.py:119-137), whose dense backward is dS cn + dS^T cn."""
+    return _SddmmFn.apply(P, Q, A)
+
+
+class _SpmmValuesFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, vals, X, A: CSR):
+        ctx.A = A
+        ctx.save_for_backward(vals, X)
+        return _spmm_new(A.with_values(vals), _f32c(X))
+
+    @staticmethod
+    def backward(ctx, g):
+        vals, X = ctx.saved_tensors
+        A, g = ctx.A, _f32c(g)
+        dv = dX = None
+        if ctx.needs_input_grad[0]:
+            dv = sddmm_raw(A, g, X)                                    # dS_e = <dY[row], X[col]>
+        if ctx.needs_input_grad[1]:
+            T, perm = A.transpose_pattern()
+            dX = _spmm_new(T.with_values(vals[perm]), g)               # dX = S^T dY
+        return dv, dX, None
+
+
+def spmm_values(A: CSR, vals: torch.Tensor, X: torch.Tensor) -> torch.Tensor:
+    """`S @ X` for the matrix S with A's pattern and the values `vals` (fp32 [nnz], CSR order), differentiable w.r.t.
+    both: dX = S^T dY on the transposed pattern (`CSR.transpose_pattern`), d vals = `sddmm_raw(A, dY, X)`.  Replaces
+    `torch.mm(item_adj, h)` on LATTICE's dense learned item graph (src/models/lattice.py:162-163)."""
+    _need_cuda(vals, X)
+    if vals.dim() != 1 or vals.numel() != A.nnz:
+        raise MMRecError(f"spmm_values: expected {A.nnz} values, got shape {tuple(vals.shape)}")
+    if X.dim() != 2 or X.shape[0] != A.n_cols:
+        raise MMRecError(f"spmm_values: X is {tuple(X.shape)}, matrix has {A.n_cols} columns")
+    return _SpmmValuesFn.apply(vals, X, A)
+
+
+def _entry_rows(A: CSR) -> torch.Tensor:
+    owner = A._owner or A
+    r = getattr(owner, "_rows64", None)
+    if r is None:
+        r = owner._rows64 = owner.coo()[0]
+    return r
+
+
+class _SymNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, vals, A: CSR):
+        ones = torch.ones(A.n_cols, 1, dtype=torch.float32, device=vals.device)
+        rowsum = _spmm_new(A.with_values(vals), ones).reshape(-1)    # ascending stored order, one fp32 add per entry
+        d = rowsum.pow(-0.5)
+        d.masked_fill_(torch.isinf(d), 0.0)                          # torch's `d_inv_sqrt[torch.isinf(d_inv_sqrt)] = 0.`
+        r, c = _entry_rows(A), A.colidx[:A.nnz].to(torch.int64)
+        ctx.A = A
+        ctx.save_for_backward(vals, rowsum, d)
+        return (d[r] * vals) * d[c]
+
+    @staticmethod
+    def backward(ctx, g):
+        vals, rowsum, d = ctx.saved_tensors
+        A, g = ctx.A, _f32c(g)
+        r, c = _entry_rows(A), A.colidx[:A.nnz].to(torch.int64)
+        # dd = S' d + S'^T d with S' = A's pattern carrying g * a: the row and column reductions, in a fixed order
+        dd = _spmm_both(A, g * vals, d.reshape(-1, 1)).reshape(-1)
+        # autograd of the reference's `pow(rowsum, -0.5)` and masked assignment: the masked entries pass 0, times -0.5 rowsum^-1.5
+        drs = torch.where(torch.isinf(rowsum.pow(-0.5)), torch.zeros_like(dd), dd) * (-0.5 * rowsum.pow(-1.5))
+        return (g * d[c]) * d[r] + drs[r], None
+
+
+def csr_sym_norm(A: CSR, vals: torch.Tensor) -> torch.Tensor:
+    """The values of D^-1/2 S D^-1/2 for the square S with A's pattern and the values `vals`: `compute_normalized_laplacian`
+    (src/utils/utils.py:126-132) on the stored entries only.  Row sums in ascending stored order (a width-1 K1 product),
+    d = rowsum^-0.5 with inf -> 0 (NaN for a negative sum), then fl(fl(d_i a_e) d_j).  Differentiable w.r.t. `vals`: the
+    row and column reductions of the backward are two width-1 K1 products, so the bits are the same on every run; where
+    the forward set d to 0 the gradient takes torch's path (0 times rowsum^-1.5)."""
+    _need_cuda(vals)
+    if A.n_rows != A.n_cols:
+        raise MMRecError(f"csr_sym_norm: the matrix must be square, got {A.n_rows} x {A.n_cols}")
+    if vals.dim() != 1 or vals.numel() != A.nnz:
+        raise MMRecError(f"csr_sym_norm: expected {A.nnz} values, got shape {tuple(vals.shape)}")
+    return _SymNormFn.apply(_f32c(vals), A)
 
 
 def propagate_mean_fused(A: CSR, ego, n_layers: int, post_csr: Optional[CSR] = None, post_x: Optional[torch.Tensor] = None,
