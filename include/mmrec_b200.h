@@ -527,6 +527,34 @@ int mmrec_late_fuse_bwd_f32(int64_t n, int d, int fusion, int weighting, const i
 int mmrec_sddmm_f32(int64_t n_rows, int64_t n_cols, int64_t nnz, const int32_t* rowptr, const int32_t* colidx,
                     const float* P, int64_t ldp, const float* Q, int64_t ldq, int d, float* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * n12  Edge attention: GRCN's graph-refining convolution.   Replaces `GATConv.message` + PyG's grouped `softmax` + the
+ * 'add' aggregation and `x + x_hat_1` (src/models/grcn.py:61-73, 158-166), which materialise x_i, x_j and the messages
+ * as [2E, d] tensors and scatter them back with atomics.
+ * The n x n CSR (rowptr, colidx) holds one entry per edge j -> i in row i (repeated edges stay separate entries); X is
+ * [n, d] (ldx), indexed by rows and columns alike.
+ *   forward:  s_e = <X[i], X[j]>, m_i = max s_e, den_i = sum expf(s_e - m_i) + 1e-16f, alpha_e = expf(s_e - m_i) / den_i,
+ *             Y[i] = base[i] + sum_e alpha_e X[j]          (base may be null: 0; alpha fp32[nnz] in CSR order)
+ *   backward: da_e = <gY[i], X[j]> + g_alpha[e] (g_alpha may be null: 0), c_i = sum alpha_e da_e,
+ *             ds_e = alpha_e (da_e - c_i), dXt[i] = sum_e ds_e X[j]
+ *   The backward's source-side terms sum_{e = (i, j)} (alpha_e gY[i] + ds_e X[i]) of dX[j] are two products of
+ *   mmrec_spmm_run_f32 on the transposed pattern; this entry point does not form them.
+ *  - Rows with at most light_max entries run on one warp; `heavy_rows` must list every longer row exactly once (longest
+ *    first balances the grid) and runs each on a CTA of 16 warps.  Per-entry scalars are parked in alpha / ds between
+ *    passes: no shared memory per entry, any row length.
+ *  - No atomics; every sum runs in an order fixed by the row's length, its light / heavy route and d: the bits are the
+ *    same on every run.  d = 64 and 128 with 16-byte aligned X / gY and ld % 4 == 0 are vectorised; any d >= 1 is
+ *    correct.  Empty rows give Y = base and touch no alpha.  Column indices must lie in [0, n) (not checked).
+ *  - A non-square matrix, bad sizes or a null pointer return MMREC_EINVAL before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+int mmrec_edge_attn_f32(int64_t n_rows, int64_t n_cols, int64_t nnz, const int32_t* rowptr, const int32_t* colidx,
+                        const float* X, int64_t ldx, int d, const float* base, int64_t ldb, const int32_t* heavy_rows,
+                        int64_t n_heavy, int light_max, float* alpha, float* Y, int64_t ldy, void* stream);
+int mmrec_edge_attn_bwd_f32(int64_t n_rows, int64_t n_cols, int64_t nnz, const int32_t* rowptr, const int32_t* colidx,
+                            const float* X, int64_t ldx, int d, const float* gY, int64_t ldg, const float* alpha,
+                            const float* g_alpha, const int32_t* heavy_rows, int64_t n_heavy, int light_max, float* ds,
+                            float* dXt, int64_t ldo, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -80,6 +80,9 @@ PROTOTYPES = {
     "mmrec_late_fuse_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _i64, _p, _p, _p, _p, _p]),
     "mmrec_late_fuse_bwd_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "mmrec_sddmm_f32": (_i32, [_i64, _i64, _i64, _p, _p, _p, _i64, _p, _i64, _i32, _p, _p]),
+    "mmrec_edge_attn_f32": (_i32, [_i64, _i64, _i64, _p, _p, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _p, _p, _i64, _p]),
+    "mmrec_edge_attn_bwd_f32": (_i32, [_i64, _i64, _i64, _p, _p, _p, _i64, _i32, _p, _i64, _p, _p, _p, _i64, _i32, _p, _p, _i64,
+                                       _p]),
 }
 
 class SpmmOp(C.Structure):

@@ -182,6 +182,33 @@ def dropout_entry_maps(inter_row, inter_col, n_users, n_items):
     return draw_of, mirror
 
 
+def grcn_edge_order(inter_row, inter_col, n_users, n_items):
+    """(rows, cols, order) of GRCN's attention graph (`src/models/grcn.py:158-159, 191-193`): the reference's symmetric edge
+    list `cat(edge_index, edge_index[[1, 0]])` with `edge_index` = the interaction COO's (u, i + n_users) pairs, edge k going
+    from source `src[k]` to target `dst[k]`, as a CSR over the targets.  Every interaction stays its own entry, as PyG sees
+    it.  CSR position e holds the reference's edge `order[e]`: a stable sort by (target, source), so repeated edges keep
+    their order.  rows = dst[order], cols = src[order] (the source node, whose `model_specific_conf` row weights the edge)."""
+    r = np.asarray(inter_row, dtype=np.int64)
+    c = np.asarray(inter_col, dtype=np.int64) + n_users
+    n = n_users + n_items
+    src, dst = np.concatenate([r, c]), np.concatenate([c, r])
+    order = np.argsort(dst * n + src, kind="stable")
+    return dst[order], src[order], order
+
+
+def build_grcn_adj(inter, n_users, n_items, device):
+    """(CSR, order int64 on the device) of `grcn_edge_order`.  The CSR build's sort is stable and the entries arrive sorted,
+    so its stored order is the host order.  Its transpose pattern and heavy-row list are built here too, so that a step can
+    be captured in a CUDA graph."""
+    r, c = (inter.row, inter.col) if hasattr(inter, "row") else inter
+    rows, cols, order = grcn_edge_order(r, c, n_users, n_items)
+    n = n_users + n_items
+    A = CSR.from_coo(_to_dev(rows, device), _to_dev(cols, device), None, n, n, sum_duplicates=False, symmetric=False)
+    A.transpose_pattern()
+    ops.edge_attention_heavy_rows(A)
+    return A, _to_dev(order, device)
+
+
 def _to_dev(a, device, dtype=None):
     t = torch.from_numpy(np.ascontiguousarray(a))
     return t.to(device=device, dtype=dtype) if dtype is not None else t.to(device)

@@ -491,6 +491,103 @@ def csr_sym_norm(A: CSR, vals: torch.Tensor) -> torch.Tensor:
     return _SymNormFn.apply(_f32c(vals), A)
 
 
+# -- n12: GRCN's edge attention (csrc/edge_attn.cu) -------------------------------------------------------------------
+EDGE_ATTN_LIGHT_MAX = 128      # rows with more entries run on a CTA of 16 warps, the others on one warp
+
+
+def edge_attention_heavy_rows(A: CSR) -> torch.Tensor:
+    """int32 list of A's rows longer than EDGE_ATTN_LIGHT_MAX, longest first (ties in row order): the rows the edge
+    attention runs on whole CTAs.  Computed once per pattern (it reads a count back, so not under CUDA graph capture) and
+    shared by every `with_values` copy."""
+    owner = A._owner or A
+    h = getattr(owner, "_attn_heavy", None)
+    if h is None:
+        _refuse_capture("edge_attention_heavy_rows")
+        deg = (owner.rowptr[1:] - owner.rowptr[:-1]).to(torch.int64)
+        rows = torch.nonzero(deg > EDGE_ATTN_LIGHT_MAX).reshape(-1)
+        rows = rows[torch.argsort(deg[rows], descending=True, stable=True)]
+        h = owner._attn_heavy = rows.to(torch.int32).contiguous()
+    return h
+
+
+def _edge_attn_args(A: CSR, X: torch.Tensor):
+    _need_cuda(X)
+    if A.n_rows != A.n_cols:
+        raise MMRecError(f"edge_attention: the matrix must be square, got {A.n_rows} x {A.n_cols}")
+    if X.dim() != 2 or X.shape[0] != A.n_rows or X.shape[1] < 1:
+        raise MMRecError(f"edge_attention: X must be [{A.n_rows}, d] with d >= 1, got {tuple(X.shape)}")
+    return _f32c(X), edge_attention_heavy_rows(A)
+
+
+def edge_attention_raw(A: CSR, X: torch.Tensor, base: Optional[torch.Tensor] = None):
+    """(Y, alpha) of `mmrec_edge_attn_f32`, no autograd: alpha = softmax over each row's entries of <X[row], X[col]>
+    (fp32 [nnz], CSR order) and Y = base + S_alpha X.  See `edge_attention`."""
+    X, heavy = _edge_attn_args(A, X)
+    n, d = X.shape
+    if base is not None:
+        _need_cuda(base)
+        if base.shape != X.shape:
+            raise MMRecError(f"edge_attention: base must be [{n}, {d}], got {tuple(base.shape)}")
+        base = _f32c(base)
+    Y = torch.empty(n, d, dtype=torch.float32, device=X.device)
+    alpha = torch.empty(max(A.nnz, 1), dtype=torch.float32, device=X.device)[:A.nnz]
+    check(_lib.load().mmrec_edge_attn_f32(A.n_rows, A.n_cols, A.nnz, _ptr(A.rowptr), _ptr(A.colidx), _ptr(X), X.stride(0), d,
+                                          _ptr(base), d, _ptr(heavy), heavy.numel(), EDGE_ATTN_LIGHT_MAX, _ptr(alpha), _ptr(Y), d,
+                                          _stream()), "mmrec_edge_attn_f32")
+    return Y, alpha
+
+
+def edge_attention_bwd_raw(A: CSR, X: torch.Tensor, gY: torch.Tensor, alpha: torch.Tensor, g_alpha: Optional[torch.Tensor] = None):
+    """(ds, dXt) of `mmrec_edge_attn_bwd_f32`: the score gradients ds (fp32 [nnz]) and the target-row part of dX."""
+    X, heavy = _edge_attn_args(A, X)
+    _need_cuda(gY, alpha, g_alpha)
+    gY, alpha = _f32c(gY), _f32c(alpha)
+    g_alpha = None if g_alpha is None else _f32c(g_alpha)
+    n, d = X.shape
+    if gY.shape != X.shape or alpha.numel() != A.nnz or (g_alpha is not None and g_alpha.numel() != A.nnz):
+        raise MMRecError("edge_attention_bwd: gY must be shaped like X, alpha and g_alpha must hold nnz values")
+    ds = torch.empty(max(A.nnz, 1), dtype=torch.float32, device=X.device)[:A.nnz]
+    dXt = torch.empty(n, d, dtype=torch.float32, device=X.device)
+    check(_lib.load().mmrec_edge_attn_bwd_f32(A.n_rows, A.n_cols, A.nnz, _ptr(A.rowptr), _ptr(A.colidx), _ptr(X), X.stride(0), d,
+                                              _ptr(gY), d, _ptr(alpha), _ptr(g_alpha), _ptr(heavy), heavy.numel(),
+                                              EDGE_ATTN_LIGHT_MAX, _ptr(ds), _ptr(dXt), d, _stream()), "mmrec_edge_attn_bwd_f32")
+    return ds, dXt
+
+
+class _EdgeAttnFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, X, base, A: CSR):
+        ctx.set_materialize_grads(False)
+        Y, alpha = edge_attention_raw(A, X, base)
+        ctx.A, ctx.has_base = A, base is not None
+        ctx.save_for_backward(X, alpha)
+        return Y, alpha
+
+    @staticmethod
+    def backward(ctx, gY, g_alpha):
+        X, alpha = ctx.saved_tensors
+        A = ctx.A
+        gY = torch.zeros_like(X) if gY is None else _f32c(gY)
+        dX = None
+        if ctx.needs_input_grad[0]:
+            ds, dXt = edge_attention_bwd_raw(A, X, gY, alpha, g_alpha)
+            T, perm = A.transpose_pattern()
+            # dX[j] += sum over the entries (i, j) of ds_e X[i] + alpha_e gY[i]: two K1 products on the transposed pattern,
+            # each adding what came before in its epilogue
+            dX = _spmm_new(T.with_values(alpha[perm]), gY, base=_spmm_new(T.with_values(ds[perm]), X, base=dXt))
+        return dX, (gY if ctx.has_base and ctx.needs_input_grad[1] else None), None
+
+
+def edge_attention(A: CSR, X: torch.Tensor, base: Optional[torch.Tensor] = None):
+    """GRCN's graph-refining convolution (`GATConv`, src/models/grcn.py:46-77, 158-166) over the square CSR A whose row i
+    holds one entry per edge j -> i: returns (Y, alpha) with alpha_e = softmax over row i of <X[i], X[j]> (PyG's grouped
+    softmax: max-shifted expf, sum + 1e-16, a division; fp32 [nnz] in CSR order) and Y = base + sum_e alpha_e X[j] (base
+    optional).  One kernel per direction (`mmrec_edge_attn_f32` / `_bwd_f32`) plus, in the backward, two K1 products on the
+    transposed pattern for the source rows.  Differentiable w.r.t. X and base, with gradients arriving through Y and
+    alpha.  No atomics: the bits are the same on every run."""
+    return _EdgeAttnFn.apply(X, base, A)
+
+
 def propagate_mean_fused(A: CSR, ego, n_layers: int, post_csr: Optional[CSR] = None, post_x: Optional[torch.Tensor] = None,
                          post_layers: int = 1, post_row0: int = 0, cooperative: bool = True) -> torch.Tensor:
     """Inference form of `propagate_mean` (+ FREEDOM / BM3's item-item term) as one `mmrec_spmm_run_f32` call:
