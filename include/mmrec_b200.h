@@ -555,6 +555,40 @@ int mmrec_edge_attn_bwd_f32(int64_t n_rows, int64_t n_cols, int64_t nnz, const i
                             const float* g_alpha, const int32_t* heavy_rows, int64_t n_heavy, int light_max, float* ds,
                             float* dXt, int64_t ldo, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * n13  Matrix-factorisation BPR loss: BPR and VBPR.   Replaces `calculate_loss` (src/models/bpr.py:67-87,
+ * src/models/vbpr.py:77-98) after the embedding tables: the three row gathers, the two row dots, `BPRLoss`
+ * (`-log(1e-10 + sigmoid(pos - neg)).mean()`), `EmbLoss` (three Frobenius norms, not squared, over B) and
+ * `mf + reg_weight * reg`, with their autograd.  VBPR's `torch.cat((i_embedding, item_linear(raw)), -1)` is not formed:
+ * the kernel reads both parts of an item row itself.
+ *   U [n_users, du] (user table), A [n_items, da] (item ID table), P [2B, dp] (projected item rows in [pos; neg] order;
+ *   NULL when dp == 0), du == da + dp >= 1.  users / pos / neg int64 [B], may repeat and need not be sorted; entries must
+ *   lie in range (not checked).  The item row of pos[b] is [A[pos[b]] | P[b]], that of neg[b] is [A[neg[b]] | P[B + b]].
+ *   forward:  x[b] = <U[users[b]], pos row> - <U[users[b]], neg row>;  norms = ||U_b||, ||Pos_b||, ||Neg_b|| (Frobenius
+ *             norms of the gathered [B, du] matrices);  loss[0] = -(sum_b logf(1e-10 + sigmoid(x[b]))) * fl(1/B)
+ *             + reg_weight * ((((0 + norms[0]) + norms[1]) + norms[2]) * fl(1/B)).  x and norms are kept for the backward.
+ *   backward: for the upstream gradient g (one fp32 on the device, read there: no host synchronisation) of loss[0]:
+ *             gU [B, du] (row b belongs to users[b]: scatter with mmrec_index_sum_rows_f32), gA_rows [2B, da] and
+ *             gP_rows [2B, dp] (the ID and projected parts of the item rows, [pos; neg]).
+ *   Rounding: every torch step is one IEEE fp32 rounding in the device's order: the mean and `/ B` multiply by fl(1/B) (as
+ *   ATen's CUDA kernels do), sigmoid is 1 / (1 + expf(-x)), its backward (g (1 - s)) s, the norm's backward
+ *   g * (x / norm) (0 where norm == 0), and the user row's gradient ((norm term + neg term) + pos term), autograd's
+ *   accumulation order.  The dots and the sums of squares run in the kernel's own fixed order: where they are exact, every
+ *   output equals the torch expression's bits.  Batch sums are per-CTA partials in ws summed by one warp in a fixed order:
+ *   the bits are the same on every run.
+ *  - One warp per row; du a multiple of 128 (64) with 16 (8)-byte aligned operands and da a multiple of 4 (2) is
+ *    vectorised; any width is correct.
+ *  - B < 1, inconsistent widths or a null pointer return MMREC_EINVAL, and a workspace below
+ *    mmrec_bpr_mf_workspace_bytes(B) MMREC_EWORKSPACE, before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+size_t mmrec_bpr_mf_workspace_bytes(int64_t B);
+int mmrec_bpr_mf_f32(int64_t B, int du, int da, int dp, const float* U, const float* A, const float* P, const int64_t* users,
+                     const int64_t* pos, const int64_t* neg, float reg_weight, float* loss, float* x, float* norms, void* ws,
+                     size_t ws_bytes, void* stream);
+int mmrec_bpr_mf_bwd_f32(int64_t B, int du, int da, int dp, const float* U, const float* A, const float* P, const int64_t* users,
+                         const int64_t* pos, const int64_t* neg, float reg_weight, const float* x, const float* norms,
+                         const float* g, float* gU, float* gA_rows, float* gP_rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -83,6 +83,9 @@ PROTOTYPES = {
     "mmrec_edge_attn_f32": (_i32, [_i64, _i64, _i64, _p, _p, _p, _i64, _i32, _p, _i64, _p, _i64, _i32, _p, _p, _i64, _p]),
     "mmrec_edge_attn_bwd_f32": (_i32, [_i64, _i64, _i64, _p, _p, _p, _i64, _i32, _p, _i64, _p, _p, _p, _i64, _i32, _p, _p, _i64,
                                        _p]),
+    "mmrec_bpr_mf_workspace_bytes": (_sz, [_i64]),
+    "mmrec_bpr_mf_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _f32, _p, _p, _p, _p, _sz, _p]),
+    "mmrec_bpr_mf_bwd_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _f32, _p, _p, _p, _p, _p, _p, _p]),
 }
 
 class SpmmOp(C.Structure):

@@ -1029,6 +1029,75 @@ def late_fuse(item_e: torch.Tensor, v: Optional[torch.Tensor], t: Optional[torch
     return _LateFuseFn.apply(item_e, v, t, alpha, idx, fu, we)
 
 
+# -- n13: BPR / VBPR's matrix-factorisation BPR loss (csrc/mf_bpr.cu) --------------------------------------------------
+def _bpr_mf_args(U, A, P, users, pos, neg):
+    """Validated, contiguous operands of `mmrec_bpr_mf_*` -- every check before anything reaches the device."""
+    if U.dim() != 2 or A.dim() != 2 or (P is not None and P.dim() != 2):
+        raise MMRecError("bpr_mf_loss: U, A and P must be 2-D")
+    for name, t in (("users", users), ("pos", pos), ("neg", neg)):
+        if t.dim() != 1 or t.dtype not in (torch.int64, torch.int32):
+            raise MMRecError(f"bpr_mf_loss: {name} must be a 1-D integer tensor")
+    B = users.numel()
+    if B < 1 or pos.numel() != B or neg.numel() != B:
+        raise MMRecError(f"bpr_mf_loss: users, pos and neg must hold the same B >= 1 entries, got {B}, {pos.numel()}, {neg.numel()}")
+    du, da = U.shape[1], A.shape[1]
+    dp = 0 if P is None else P.shape[1]
+    if du != da + dp or du < 1:
+        raise MMRecError(f"bpr_mf_loss: U is {du} wide, the item rows [A | P] {da} + {dp}")
+    if P is not None and P.shape[0] != 2 * B:
+        raise MMRecError(f"bpr_mf_loss: P must hold the 2B = {2 * B} projected rows [pos; neg], got {P.shape[0]}")
+    _need_cuda(U, A, P, users, pos, neg)
+    idx = [t.to(torch.int64).contiguous() for t in (users, pos, neg)]
+    return _f32c(U), _f32c(A), None if P is None else _f32c(P), idx, B, du, da, dp
+
+
+class _BprMfFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, U, A, P, users, pos, neg, reg_weight: float):
+        lib = _lib.load()
+        B, du, da = users.numel(), U.shape[1], A.shape[1]
+        dp = 0 if P is None else P.shape[1]
+        dev = U.device
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        x = torch.empty(B, dtype=torch.float32, device=dev)
+        norms = torch.empty(3, dtype=torch.float32, device=dev)
+        ws = _ws("bpr_mf", lib.mmrec_bpr_mf_workspace_bytes(B), dev)
+        check(lib.mmrec_bpr_mf_f32(B, du, da, dp, _ptr(U), _ptr(A), _ptr(P), _ptr(users), _ptr(pos), _ptr(neg), float(reg_weight),
+                                   _ptr(loss), _ptr(x), _ptr(norms), _ptr(ws), ws.numel(), _stream()), "mmrec_bpr_mf_f32")
+        ctx.save_for_backward(U, A, P, users, pos, neg, x, norms)
+        ctx.reg_weight = float(reg_weight)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        U, A, P, users, pos, neg, x, norms = ctx.saved_tensors
+        B, du, da = users.numel(), U.shape[1], A.shape[1]
+        dp = 0 if P is None else P.shape[1]
+        g = _f32c(g.reshape(1))
+        gU = torch.empty(B, du, dtype=torch.float32, device=U.device)
+        gA = torch.empty(2 * B, da, dtype=torch.float32, device=U.device)
+        gP = None if P is None else torch.empty(2 * B, dp, dtype=torch.float32, device=U.device)
+        check(_lib.load().mmrec_bpr_mf_bwd_f32(B, du, da, dp, _ptr(U), _ptr(A), _ptr(P), _ptr(users), _ptr(pos), _ptr(neg),
+                                               ctx.reg_weight, _ptr(x), _ptr(norms), _ptr(g), _ptr(gU), _ptr(gA), _ptr(gP),
+                                               _stream()), "mmrec_bpr_mf_bwd_f32")
+        dU = index_sum_rows(gU, users, U.shape[0]) if ctx.needs_input_grad[0] else None   # ascending j: bit-reproducible
+        dA = index_sum_rows(gA, torch.cat((pos, neg)), A.shape[0]) if ctx.needs_input_grad[1] else None
+        return dU, dA, gP, None, None, None, None
+
+
+def bpr_mf_loss(U: torch.Tensor, A: torch.Tensor, P: Optional[torch.Tensor], users: torch.Tensor, pos: torch.Tensor,
+                neg: torch.Tensor, reg_weight: float) -> torch.Tensor:
+    """BPR / VBPR's `calculate_loss` after the tables (`src/models/bpr.py:67-87`, `src/models/vbpr.py:77-98`): the
+    [1]-shaped `BPRLoss(pos_score, neg_score) + reg_weight * EmbLoss(user_e, pos_e, neg_e)` of the rows `U[users]`,
+    `[A[pos] | P[:B]]` and `[A[neg] | P[B:]]`, in one kernel each way (`mmrec_bpr_mf_f32` / `_bwd_f32`), differentiable
+    w.r.t. U, A and P.  `P` holds the 2B projected item rows in [pos; neg] order (VBPR: `project(raw, W, b,
+    idx=cat(pos, neg))`), or is None (BPR).  The table gradients are the per-row gradients scattered by `index_sum_rows`.
+    Every element-wise step is the torch expression's on the device, so where the dots and norms are exact the loss and
+    gradients equal its bits; the batch sums are the same bits on every run.  Never synchronises with the host."""
+    U, A, P, (users, pos, neg), B, du, da, dp = _bpr_mf_args(U, A, P, users, pos, neg)
+    return _BprMfFn.apply(U, A, P, users, pos, neg, float(reg_weight))
+
+
 # ------------------------------------------------------------------------------------------------
 # K3: scoring, mask, top-k
 # ------------------------------------------------------------------------------------------------
