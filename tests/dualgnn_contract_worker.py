@@ -1,94 +1,34 @@
-"""Worker of tests/test_dualgnn_contract.py (own process: the kernels behind `mmrec_b200.ops` are patched).
-
-DualGNN (`mmrec_b200.models.dualgnn`) under the harness of tests/dropin_contract_worker.py -- built the way quick_start
-builds it, the package's restatement or, with MMREC_REFERENCE_SRC, the reference's own code -- with the kernels replaced by
-`install_cpu_ops`'s CPU stand-ins plus one for `ops.propagate_sum` (the reference's `h = A x`, `h_1 = A h`, `h + x + h_1`
-with `torch.sparse.mm`), against tests/golden/dualgnn_tiny.npz / traj_dualgnn_tiny.npz recorded from the reference's class.
-The dataset's `user_graph_dict.npy` is written by `synth.write_user_graph_dict`."""
-import json
-import os
+"""Worker of tests/test_dualgnn_contract.py: DualGNN (`mmrec_b200.models.dualgnn`) under the harness of tests/contract.py,
+with `install_cpu_ops`'s CPU stand-ins plus `contract.propagate_sum`, against tests/golden/dualgnn_tiny.npz /
+traj_dualgnn_tiny.npz recorded from the reference's class.  The dataset's `user_graph_dict.npy` is written by
+`synth.write_user_graph_dict`."""
 import sys
-import tempfile
 
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.dirname(HERE))
-sys.path.insert(0, os.path.join(HERE, "golden"))
-sys.path.insert(0, HERE)
+import contract as C
+import dualgnn_golden as D
+import golden_io as G
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
-from dropin_contract_worker import harness, install_cpu_ops  # noqa: E402
+AFTER = {"user_graph_dict_file": "user_graph_dict.npy"}
 
 
-def _setup(epochs=None, text_only=False):
-    from mmrec_b200.utils import synth
-    torch.set_num_threads(1)
-    tmp = tempfile.mkdtemp(prefix="mmrec_contract_")
-    data, Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra = harness(tmp)
-    u, i, e, d, f = synth.SHAPES["tiny"]
-    g = synth.make_graph(u, i, e, seed=0)
-    v, t = synth.make_features(i, f, seed=1)
-    synth.write_dataset(data, "tiny", g, None if text_only else v, t)
-    synth.write_user_graph_dict(data, "tiny", g)
-    over = {"gpu_id": 0, "use_gpu": False, "eval_batch_size": 128, "train_batch_size": 512}
-    config = Config("DualGNN", "tiny", dict(over, **extra))
-    config["inter_file_name"] = "tiny.inter"
-    config["USER_ID_FIELD"], config["ITEM_ID_FIELD"] = "userID", "itemID"
-    config["vision_feature_file"], config["text_feature_file"] = "image_feat.npy", "text_feat.npy"
-    config["user_graph_dict_file"] = "user_graph_dict.npy"
-    for k in config["hyper_parameters"]:
-        if isinstance(config[k], list):
-            config[k] = config[k][0]
-    if epochs:
-        config["epochs"] = epochs
-    dataset = RecDataset(config)
-    str(dataset)
-    tr, va, te = dataset.split()
-    str(tr), str(va), str(te)
-    train_data = TrainDataLoader(config, tr, batch_size=config["train_batch_size"], shuffle=True)
-    valid_data = EvalDataLoader(config, va, additional_dataset=tr, batch_size=config["eval_batch_size"])
-    test_data = EvalDataLoader(config, te, additional_dataset=tr, batch_size=config["eval_batch_size"])
-    init_seed(config["seed"])
-    train_data.pretrain_setup()
-    install_cpu_ops()
+def install():
     from mmrec_b200 import ops
-
-    def propagate_sum(A, ego, n_layers):
-        out, x = ego, ego
-        for _ in range(n_layers):
-            x = torch.sparse.mm(A.t_, x)
-            out = x + out if out is ego else out + x                     # (h + x) + h_1, dualgnn.py:314
-        return out
-    ops.propagate_sum = propagate_sum
-    from mmrec_b200.models.dualgnn import DualGNN
-    model = DualGNN(config, train_data).to(config["device"])
-    return config, model, valid_data, test_data, Trainer
+    ops.propagate_sum = C.propagate_sum
 
 
 def main_model(p=""):
-    config, model, valid_data, test_data, Trainer = _setup(text_only=p == "text.")
-    gold = np.load(os.path.join(HERE, "golden", "dualgnn_tiny.npz"), allow_pickle=True)
-    sub = {k[len(p):]: gold[k] for k in gold.files if k.startswith(p)} if p else {k: gold[k] for k in gold.files}
-    init = {k: v for k, v in sub.items() if k.startswith("init_sha256.")}
-
-    class _G:
-        files = list(init)
-
-        def __getitem__(self, k):
-            return init[k]
-    out = {"init_identical": not selfcf_golden.same_init(model, _G())
-           and [k for k, _ in model.named_parameters()] == [str(x) for x in sub["param_order"]]
-           and G.sha256(model.result_embed.numpy()) == str(sub["result_embed0_sha256"]),
+    h = C.build("DualGNN", "t" if p == "text." else "vt", user_graph=True, after=AFTER, install=install)
+    model, sub = h.model, C.case(C.load("dualgnn_tiny.npz"), p)
+    out = {"init_identical": C.check_init(model, sub) and G.sha256_tagged(model.result_embed.numpy()) == str(sub["result_embed0_sha256"]),
            "has_v_gcn": hasattr(model, "v_gcn")}
-    eb = [torch.from_numpy(sub["eval_users"]), torch.from_numpy(sub["eval_mask"])]
     model.eval()
     with torch.no_grad():
-        s0 = model.full_sort_predict(eb)
+        s0 = model.full_sort_predict([torch.from_numpy(sub["eval_users"]), torch.from_numpy(sub["eval_mask"])])
     out["scores0_equal"] = bool(s0.dtype == torch.float64 and G.equal(sub, "scores0", s0.numpy()))
-    np.random.seed(G.SAMPLE_SEED)
+    np.random.seed(D.SAMPLE_SEED)
     model.pre_epoch_processing()
     out["sample_equal"] = bool(G.equal(sub, "sample_idx", model.epoch_user_graph.numpy())
                                and G.equal(sub, "sample_w", model.user_weight_matrix.numpy()))
@@ -109,53 +49,18 @@ def main_model(p=""):
     out["user_rep_rel"] = G.rel(sub, "user_rep", seen["user_rep"])
     out["result_embed_rel"] = G.rel(sub, "result_embed", model.result_embed.detach().numpy())
     loss.backward()
-    named = dict(model.named_parameters())
-    grads = [k[5:] for k in G.recorded(sub, "grad.")]
-    out.update({"loss": float(loss.item()), "want_loss": float(sub["loss"][0]),
-                "grad_keys": sorted(k for k, q in named.items() if q.grad is not None) == grads,
-                "grad_rel": {k: G.rel(sub, "grad." + k, named[k].grad.numpy()) for k in grads}})
+    out["grad_keys"], out["grad_rel"] = C.check_grads(model, sub)
+    out.update({"loss": float(loss.item()), "want_loss": float(sub["loss"][0])})
     model.zero_grad()
-    model.eval()
-    with torch.no_grad():
-        sc = model.full_sort_predict(eb)
-    out["score_rel"] = G.rel(sub, "scores", sc.numpy())
-    trainer = Trainer(config, model)
-    valid = trainer.evaluate(valid_data)
-    test = trainer.evaluate(test_data, is_test=True)
-    names = [str(x) for x in sub["metric_names"]]
-    out.update({"valid": {k: float(v) for k, v in valid.items()}, "want_valid": dict(zip(names, [float(x) for x in sub["metric_values"]])),
-                "test": {k: float(v) for k, v in test.items()}, "want_test": dict(zip(names, [float(x) for x in sub["test_metric_values"]]))})
-    print("CONTRACT " + json.dumps(out))
+    out["score_rel"] = G.rel(sub, "scores", C.predict(model, sub))
+    out.update(C.check_metrics(h, sub))
+    C.emit(out)
 
 
 def main_traj():
-    config, model, valid_data, test_data, Trainer = _setup(epochs=2)
-    gold = np.load(os.path.join(HERE, "golden", "traj_dualgnn_tiny.npz"), allow_pickle=True)
-    trainer = Trainer(config, model)
-    rec = {"losses": [], "valid": [], "test": []}
-    orig = model.calculate_loss
-
-    def spy(interaction):
-        l = orig(interaction)
-        rec["losses"].append(float(l.detach()))
-        return l
-    model.calculate_loss = spy
-    offs = np.concatenate([[0], np.cumsum(gold["batch_sizes"])])
-    first = np.concatenate([[0], np.cumsum(gold["batches_per_epoch"])])
-    batches = gold["batches"]
-    recorded = [[torch.from_numpy(batches[:, offs[b]:offs[b + 1]].copy()) for b in range(first[ep], first[ep + 1])]
-                for ep in range(len(gold["batches_per_epoch"]))]
-    for ep in range(2):
-        np.random.seed(int(gold["epoch_seed0"]) + ep)
-        model.pre_epoch_processing()
-        trainer._train_epoch(recorded[ep], ep)
-        trainer.lr_scheduler.step()
-        rec["valid"].append(list(trainer.evaluate(valid_data).values()))
-        rec["test"].append(list(trainer.evaluate(test_data, is_test=True).values()))
-    out = {"n_batches": len(rec["losses"]), "want_batches": int(gold["n_steps"]),
-           "loss_max_rel": float(np.max(np.abs(np.array(rec["losses"]) - gold["losses"]) / np.abs(gold["losses"]))),
-           "metric_max_abs": float(max(np.abs(np.array(rec["valid"]) - gold["valid"]).max(), np.abs(np.array(rec["test"]) - gold["test"]).max()))}
-    print("CONTRACT " + json.dumps(out))
+    h = C.build("DualGNN", user_graph=True, after=dict(AFTER, epochs=2), install=install)
+    gold = C.load("traj_dualgnn_tiny.npz")
+    C.emit(C.replay_trajectory(h, gold, lambda ep: np.random.seed(int(gold["epoch_seed0"]) + ep)))
 
 
 if __name__ == "__main__":

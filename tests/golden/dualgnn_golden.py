@@ -1,14 +1,6 @@
-"""Shared by DualGNN's golden generator (make_golden_dualgnn.py) and its tests: the recorded graphs, the seeds, the
-`user_graph_dict` as flat arrays (`ptr` [U + 1], `idx`, `val`: user u's neighbours are idx[ptr[u]:ptr[u + 1]]), and how a
-recorded tensor is kept.
-
-A tensor is kept as the SHA-256 of its bytes (`<key>.sha256`: bit equality) and, for comparisons within a tolerance,
-either whole (`<key>`: up to SMALL elements, or where the file names it so) or as a sketch (`<key>.sketch`): its rows
-times a fixed Gaussian matrix of SKETCH_COLS columns, computed in float64 and stored as fp32.  A random projection keeps
-the norm of a difference to within a small factor, so the relative error of the sketches stands for the relative error of
-the tensors, and a [256, 128] gradient takes 16 KiB instead of 128 KiB of incompressible bytes."""
-import hashlib
-
+"""Shared by DualGNN's golden generator (make_golden_dualgnn.py) and its tests: the recorded graphs, the seeds, and the
+`user_graph_dict` as flat arrays (`ptr` [U + 1], `idx`, `val`: user u's neighbours are idx[ptr[u]:ptr[u + 1]]).  How a
+recorded tensor is kept: golden_io.py."""
 import numpy as np
 
 # synth.make_graph(users, items, train interactions, seed) of the two graphs the preprocessing script was run on:
@@ -18,58 +10,6 @@ SAMPLE_SEED = 2024            # np.random.seed before the recorded `pre_epoch_pr
 BATCH_SEED = 7
 EPOCH_SEED0 = 3000            # np.random.seed(EPOCH_SEED0 + epoch) before each trajectory epoch's `pre_epoch_processing`
 K = 40
-
-
-def sha256(a) -> str:
-    """SHA-256 of the array's bytes in its own dtype (float64 stays float64)."""
-    a = np.ascontiguousarray(a)
-    return hashlib.sha256(a.dtype.str.encode() + a.tobytes()).hexdigest()
-
-
-SMALL = 4096
-SKETCH_COLS = 16
-
-
-def sketch(a) -> np.ndarray:
-    a = np.asarray(a, dtype=np.float64)
-    a = a.reshape(a.shape[0], -1)
-    R = np.random.default_rng(a.shape[1]).standard_normal((a.shape[1], SKETCH_COLS))
-    return (a @ R).astype(np.float32)
-
-
-def put_sha(g: dict, key: str, a):
-    g[key + ".sha256"] = np.array(sha256(a))
-
-
-def put(g: dict, key: str, a, whole: bool = False):
-    """Record `a` under `key`: its digest, and the tensor itself or its sketch."""
-    a = np.asarray(a)
-    put_sha(g, key, a)
-    if whole or a.size <= SMALL:
-        g[key] = a.copy()
-    else:
-        g[key + ".sketch"] = sketch(a)
-
-
-def equal(gold, key, a) -> bool:
-    """`a` has the recorded bits (dtype and shape included)."""
-    return sha256(np.asarray(a)) == str(gold[key + ".sha256"])
-
-
-def rel(gold, key, a) -> float:
-    """Relative 2-norm difference of `a` from the recorded tensor, or of their sketches."""
-    a = np.asarray(a, dtype=np.float64)
-    if key in gold:
-        ref, got = np.asarray(gold[key], dtype=np.float64), a
-    else:
-        ref, got = np.asarray(gold[key + ".sketch"], dtype=np.float64), sketch(a)
-    return float(np.linalg.norm(got - ref) / max(np.linalg.norm(ref), 1e-30))
-
-
-def recorded(gold, prefix: str) -> list:
-    """The keys recorded under `prefix` (e.g. "grad."), without the `.sha256` / `.sketch` suffixes."""
-    keys = {str(k) for k in (gold.files if hasattr(gold, "files") else gold)}
-    return sorted({k[:-len(".sha256")] for k in keys if k.startswith(prefix) and k.endswith(".sha256")})
 
 
 def flatten(d: dict):

@@ -10,15 +10,12 @@ draws themselves are regenerated from a CPU `torch.Generator` with that seed: th
 CPU generator seeded the same way and consumed by nothing else within the phase, which make_golden_lgmrec.py asserts by
 regenerating every phase and comparing the digests.  (Storing the noise itself would take 4 incompressible bytes per
 element: over 2 MB for the H = 64 setting.)"""
-import hashlib
 import os
 
 import numpy as np
 import torch
 
-
-def digest(a) -> str:
-    return hashlib.sha256(np.ascontiguousarray(a, dtype=np.float32).tobytes()).hexdigest()
+from golden_io import sha256_fp32
 
 
 def pack(prefix, seed, specs, draws) -> dict:
@@ -26,7 +23,7 @@ def pack(prefix, seed, specs, draws) -> dict:
     assert len(specs) == len(draws) and all(len(s[1]) == 2 for s in specs)
     return {prefix + "seed": np.int64(seed), prefix + "n_draws": np.int64(len(specs)),
             prefix + "draw_kind": np.array([s[0] for s in specs]), prefix + "draw_shape": np.array([s[1] for s in specs], dtype=np.int64).reshape(-1, 2),
-            prefix + "draw_p": np.array([s[2] for s in specs], dtype=np.float64), prefix + "draw_sha256": np.array([digest(a) for a in draws])}
+            prefix + "draw_p": np.array([s[2] for s in specs], dtype=np.float64), prefix + "draw_sha256": np.array([sha256_fp32(a) for a in draws])}
 
 
 def regenerate(gold, prefix):
@@ -41,7 +38,7 @@ def regenerate(gold, prefix):
             x = torch.empty(shape).bernoulli_(1 - p, generator=gen)
             x.div_(1 - p)
         a = x.numpy()
-        assert digest(a) == str(gold[prefix + "draw_sha256"][k]), f"{prefix}draw {k}: torch's CPU generator no longer gives the recorded draw"
+        assert sha256_fp32(a) == str(gold[prefix + "draw_sha256"][k]), f"{prefix}draw {k}: torch's CPU generator no longer gives the recorded draw"
         out.append(a)
     return out
 

@@ -11,7 +11,7 @@ only where `.to` returns its argument, on the CPU; on the GPU `.to` returns a pl
 fresh data directory, so the constructor builds `mm_adj` instead of loading a `mm_adj_{k}.pt` left by another run.
 
 Recorded (dragon_tiny.npz), each tensor as its SHA-256 and, where a tolerance applies, whole or as a fixed random sketch
-(dualgnn_golden.put): the initial state as one SHA-256 per `state_dict` entry and of the float64 `result_embed`, the
+(golden_io.put): the initial state as one SHA-256 per `state_dict` entry and of the float64 `result_embed`, the
 parameter order, four `np.random` and four `torch` draws taken right after construction (`rng_after_*`: the
 construction's RNG consumption), the coalesced `mm_adj` (indices and values), the seeded `pre_epoch_processing` sample;
 on one batch in training mode `user_rep` before the user graph, `result_embed`, the mutated batch, the loss and every
@@ -32,10 +32,10 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
+import dualgnn_golden as D  # noqa: E402
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
-import selfcf_golden  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 COMMON = {"eval_batch_size": 128, "train_batch_size": 512, "user_graph_dict_file": "user_graph_dict.npy"}
@@ -72,10 +72,10 @@ def dump_model(g, prefix, overrides):
         for k in ("embedding_size", "reg_weight", "learning_rate", "train_batch_size", "knn_k", "mm_image_weight", "n_mm_layers"):
             g["cfg_" + k] = np.float64(config[k])
     g[p + "cfg_aggr_mode"] = np.array(config["aggr_mode"])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g[p + "init_sha256." + k] = np.array(v)
     assert model.result_embed.dtype == torch.float64
-    g[p + "result_embed0_sha256"] = np.array(G.sha256(model.result_embed.numpy()))
+    g[p + "result_embed0_sha256"] = np.array(G.sha256_tagged(model.result_embed.numpy()))
     g[p + "param_order"] = np.array([k for k, _ in model.named_parameters()])
     mm = model.mm_adj.coalesce()
     g[p + "mm_adj_indices"] = mm.indices().numpy().copy()
@@ -89,12 +89,12 @@ def dump_model(g, prefix, overrides):
         assert s0.dtype == torch.float64
         G.put_sha(g, p + "scores0", s0.numpy())
         g[p + "scores0_rows"] = s0[:SCORE_ROWS].numpy().copy()
-    np.random.seed(G.SAMPLE_SEED)
+    np.random.seed(D.SAMPLE_SEED)
     model.pre_epoch_processing()
     G.put_sha(g, p + "sample_idx", np.array(model.epoch_user_graph, dtype=np.int64))
     G.put_sha(g, p + "sample_w", model.user_weight_matrix.numpy())
     import random
-    random.seed(G.BATCH_SEED); np.random.seed(G.BATCH_SEED)
+    random.seed(D.BATCH_SEED); np.random.seed(D.BATCH_SEED)
     batch = next(iter(train_data))
     train_data.pr = 0
     g[p + "batch"] = batch.numpy().copy()
@@ -150,7 +150,7 @@ def dump_trajectory(out, epochs=2):
     model.calculate_loss = spy
     batch_epoch = []
     for ep in range(epochs):
-        np.random.seed(G.EPOCH_SEED0 + ep)
+        np.random.seed(D.EPOCH_SEED0 + ep)
         model.pre_epoch_processing()
         n0 = len(rec["batches"])
         trainer._train_epoch(train_data, ep)
@@ -162,7 +162,7 @@ def dump_trajectory(out, epochs=2):
          "batches_per_epoch": np.array(batch_epoch), "losses": np.array(rec["losses"], dtype=np.float64),
          "valid": np.array(rec["valid"], dtype=np.float64), "test": np.array(rec["test"], dtype=np.float64),
          "learning_rate": np.float64(config["learning_rate"]), "n_steps": np.int64(len(rec["losses"])),
-         "epoch_seed0": np.int64(G.EPOCH_SEED0)}
+         "epoch_seed0": np.int64(D.EPOCH_SEED0)}
     g["metric_names"] = np.array(list(trainer.evaluate(valid_data).keys()))
     np.savez_compressed(out, **g)
     print(f"trajectory DRAGON: {len(rec['losses'])} batches, loss {rec['losses'][0]:.6f} -> {rec['losses'][-1]:.6f}")

@@ -17,7 +17,7 @@
    a parameter's name).
 
 Recorded (dualgnn_tiny.npz), each tensor as its SHA-256 and, where a tolerance applies, whole or as a fixed random
-sketch (dualgnn_golden.put): both user-graph dicts (digests of their flat arrays); the initial state as one SHA-256 per
+sketch (golden_io.put): both user-graph dicts (digests of their flat arrays); the initial state as one SHA-256 per
 `state_dict` entry and of the float64 `result_embed`, and the parameter order; the seeded `pre_epoch_processing` sample
 (index and weights); on one batch in training mode `v_rep` / `t_rep` after the in-place add, `user_rep` before the user
 graph, `result_embed` (whole), the mutated batch, the loss and every gradient; the float64 scores before any forward
@@ -41,10 +41,10 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
+import dualgnn_golden as D  # noqa: E402
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
-import selfcf_golden  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 COMMON = {"eval_batch_size": 128, "train_batch_size": 512, "user_graph_dict_file": "user_graph_dict.npy"}
@@ -52,7 +52,7 @@ SCORE_ROWS = 16
 
 
 def graph_of(name):
-    return synth.named(name) if G.GRAPHS[name] is None else synth.make_graph(*G.GRAPHS[name])
+    return synth.named(name) if D.GRAPHS[name] is None else synth.make_graph(*D.GRAPHS[name])
 
 
 def run_script(tmp, name, graph):
@@ -89,10 +89,10 @@ def dump_model(g, prefix):
         for k in ("embedding_size", "reg_weight", "learning_rate", "train_batch_size"):
             g["cfg_" + k] = np.float64(config[k])
         g["cfg_aggr_mode"] = np.array(config["aggr_mode"])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g[p + "init_sha256." + k] = np.array(v)
     assert model.result_embed.dtype == torch.float64
-    g[p + "result_embed0_sha256"] = np.array(G.sha256(model.result_embed.numpy()))
+    g[p + "result_embed0_sha256"] = np.array(G.sha256_tagged(model.result_embed.numpy()))
     g[p + "param_order"] = np.array([k for k, _ in model.named_parameters()])
     model.eval()
     with torch.no_grad():                                           # before any forward: the float64 initial table
@@ -103,12 +103,12 @@ def dump_model(g, prefix):
         assert s0.dtype == torch.float64
         G.put_sha(g, p + "scores0", s0.numpy())
         g[p + "scores0_rows"] = s0[:SCORE_ROWS].numpy().copy()
-    np.random.seed(G.SAMPLE_SEED)
+    np.random.seed(D.SAMPLE_SEED)
     model.pre_epoch_processing()
     G.put_sha(g, p + "sample_idx", np.array(model.epoch_user_graph, dtype=np.int64))
     G.put_sha(g, p + "sample_w", model.user_weight_matrix.numpy())
     import random
-    random.seed(G.BATCH_SEED); np.random.seed(G.BATCH_SEED)
+    random.seed(D.BATCH_SEED); np.random.seed(D.BATCH_SEED)
     batch = next(iter(train_data))
     train_data.pr = 0
     g[p + "batch"] = batch.numpy().copy()
@@ -167,7 +167,7 @@ def dump_trajectory(out, epochs=2):
     model.calculate_loss = spy
     batch_epoch = []
     for ep in range(epochs):
-        np.random.seed(G.EPOCH_SEED0 + ep)
+        np.random.seed(D.EPOCH_SEED0 + ep)
         model.pre_epoch_processing()
         n0 = len(rec["batches"])
         trainer._train_epoch(train_data, ep)
@@ -179,7 +179,7 @@ def dump_trajectory(out, epochs=2):
          "batches_per_epoch": np.array(batch_epoch), "losses": np.array(rec["losses"], dtype=np.float64),
          "valid": np.array(rec["valid"], dtype=np.float64), "test": np.array(rec["test"], dtype=np.float64),
          "learning_rate": np.float64(config["learning_rate"]), "n_steps": np.int64(len(rec["losses"])),
-         "epoch_seed0": np.int64(G.EPOCH_SEED0)}
+         "epoch_seed0": np.int64(D.EPOCH_SEED0)}
     g["metric_names"] = np.array(list(trainer.evaluate(valid_data).keys()))
     np.savez_compressed(out, **g)
     print(f"trajectory DualGNN: {len(rec['losses'])} batches, loss {rec['losses'][0]:.6f} -> {rec['losses'][-1]:.6f}")
@@ -194,10 +194,10 @@ def main():
     tmp = tempfile.mkdtemp(prefix="mmrec_golden_")
     g = {}
     files = {}
-    for name in G.GRAPHS:
+    for name in D.GRAPHS:
         files[name] = run_script(tmp, name, graph_of(name))
         d = np.load(files[name], allow_pickle=True).item()
-        for part, a in zip(("ptr", "idx", "val"), G.flatten(d)):
+        for part, a in zip(("ptr", "idx", "val"), D.flatten(d)):
             G.put_sha(g, "ugd_%s_%s" % (name, part), a)
     u, i, e, dim, f = synth.SHAPES[make_golden.DATASET]
     graph = graph_of("tiny")

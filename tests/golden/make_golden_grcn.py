@@ -19,7 +19,7 @@ state after construction; `full_sort_predict` of the first validation batch befo
 on one training batch the final convolution's alpha of each modality and the edge weight in the reference's edge order
 (`cat(edge_index, edge_index[[1, 0]])`), `forward`'s representation, the loss and every gradient; then, in evaluation,
 `full_sort_predict` of the first validation batch (the batch's representation), the trainer's top-50 of it and the
-validation and test metrics.  Tensors above 4096 elements are kept as digest and sketch (`dualgnn_golden.put`).
+validation and test metrics.  Tensors above 4096 elements are kept as digest and sketch (`golden_io.put`).
 Cases: both modalities at n_layers 3 (the config's, no prefix) and 1 (`l1.`), image only (`image.`).
 traj_grcn_tiny.npz: two epochs of the reference's Trainer (both modalities, learning rate 0.001: the config's first grid
 value, 1, makes Adam's steps chaotic) with its batches, losses and metrics."""
@@ -38,10 +38,9 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
-import selfcf_golden  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 COMMON = {"eval_batch_size": 128, "train_batch_size": 512}
@@ -122,7 +121,7 @@ def dump_model(g, prefix, overrides):
         for k in ("embedding_size", "latent_embedding", "reg_weight", "learning_rate", "train_batch_size"):
             g["cfg_" + k] = np.float64(config[k])
     g[p + "cfg_n_layers"] = np.int64(config["n_layers"])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g[p + "init_sha256." + k] = np.array(v)
     g[p + "param_order"] = np.array([k for k, _ in model.named_parameters()])
 

@@ -13,7 +13,7 @@ Recorded (lattice_tiny.npz), per case: the SHA-256 of every initial `state_dict`
 next batch (the stored graph, detached) the loss and every gradient; then in evaluation `full_sort_predict` of the first
 validation batch, the trainer's top-50 of it and the validation and test metrics.  The `item_adj` evaluation leaves behind
 is the graph-building batch's bit for bit (no optimizer step in between; asserted here), so it is not recorded twice.
-Tensors of more than 4096 elements are kept as digest and sketch (`dualgnn_golden.put`), indices as int32 (the top-50
+Tensors of more than 4096 elements are kept as digest and sketch (`golden_io.put`), indices as int32 (the top-50
 as int16).  To keep the file small, `forward`'s embeddings and the ordinary batch's gradients are recorded for the first
 case only (the others record that batch's loss), and a case's learned graph only where it differs from the first case's
 (lightgcn at two layers and mf draw the same initial weights, so they build the same graph).
@@ -34,10 +34,9 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
-import selfcf_golden  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 COMMON = {"eval_batch_size": 128, "train_batch_size": 512}
@@ -74,7 +73,7 @@ def dump_model(g, prefix, overrides):
         g["norm_adj_indices"], g["norm_adj_values"] = na.indices().numpy().astype(np.int32), na.values().numpy().copy()
     g[p + "cfg_cf_model"] = np.array(config["cf_model"])
     g[p + "cfg_n_layers"] = np.int64(config["n_layers"])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g[p + "init_sha256." + k] = np.array(v)
     g[p + "param_order"] = np.array([k for k, _ in model.named_parameters()])
     if not prefix:                                                  # the same features in every case

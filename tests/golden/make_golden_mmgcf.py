@@ -5,7 +5,7 @@
 The unmodified model class (`src/models/mmgcf.py`) runs under the harness, dataset and fields of make_golden.py (`tiny`,
 `train_batch_size` 512), with no shim.  For every case of `CASES` (all nine fusion_mode x weighting pairs with both
 modalities, two pairs text-only; n_ui_layers 1 or 2) mmgcf_tiny.npz keeps, under the case's name as prefix, each tensor as
-its SHA-256 and, where a tolerance applies, whole or as a fixed random sketch (dualgnn_golden.put):
+its SHA-256 and, where a tolerance applies, whole or as a fixed random sketch (golden_io.put):
 - the initial state, one SHA-256 per `state_dict` entry, and the parameter order;
 - once for all cases (they are the same): `norm_adj` and the masked adjacency (digests of the COO indices, values whole),
   `edge_values`, and the pruning draw (`torch.multinomial` with torch seeded PRUNE_SEED, recorded from a saved RNG state
@@ -31,10 +31,9 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
-import selfcf_golden  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 COMMON = {"eval_batch_size": 128, "train_batch_size": 512}
@@ -72,7 +71,7 @@ def dump_case(g, name):
     config, train_data, valid_data, test_data, model = make_golden.build("MMGCF", overrides(fusion, weighting, layers))
     p = name + "."
     g[p + "cfg"] = np.array([fusion, weighting, str(layers), str(config["dropout"]), str(config["reg_weight"])])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g[p + "init_sha256." + k] = np.array(v)
     g[p + "param_order"] = np.array([k for k, _ in model.named_parameters()])
     torch.manual_seed(PRUNE_SEED)

@@ -7,7 +7,7 @@ it uses -- `MessagePassing`, `remove_self_loops`, `add_self_loops`, `degree`, `i
 documented behaviour, as for MMGCN).  Same harness, dataset (`tiny`) and fields as make_golden.py's `dump_model`, with
 `train_batch_size` 512, except where that would make the file large:
 - the initial state (the `state_dict` and the plain tensors the reference keeps beside its parameters: `collaborative`,
-  each GCN's `preference`, the initial `result_embed`) is kept as one SHA-256 per tensor (`mvgae_golden.init_digests`: bit
+  each GCN's `preference`, the initial `result_embed`) is kept as one SHA-256 per tensor (`golden_io.init_digests`: bit
   for bit, without 1.2 MiB of incompressible weights);
 - the forward keeps its output `pd_mu`, the precision-weighted mean of the experts, which every tower's mu and logvar enter
   (in evaluation mode z is pd_mu; pd_logvar enters the recorded loss and gradients);
@@ -37,6 +37,8 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
+import golden_io as G  # noqa: E402
+import lgmrec_golden  # noqa: E402
 import make_golden  # noqa: E402
 import mvgae_golden  # noqa: E402
 import ref_loader  # noqa: E402
@@ -57,7 +59,7 @@ class Recorder:
 
     def take(self, g, prefix, seed):
         """Store the phase drawn since the last call under `prefix`, after checking that it regenerates from `seed`."""
-        g.update(mvgae_golden.pack(prefix, seed, self.specs, self.draws))
+        g.update(lgmrec_golden.pack(prefix, seed, self.specs, self.draws))
         again = mvgae_golden.regenerate(g, prefix)
         assert len(again) == len(self.draws) and all(np.array_equal(a, b) for a, b in zip(again, self.draws)), prefix
         self.draws, self.specs = [], []
@@ -113,7 +115,7 @@ def dump_mvgae(out):
     for k in ("embedding_size", "n_layers", "beta", "train_batch_size", "learning_rate"):
         g["cfg_" + k] = np.float64(config[k])
     g["edge_index"] = model.edge_index.numpy().copy()
-    for k, v in mvgae_golden.init_digests(model).items():
+    for k, v in G.init_digests(model, mvgae_golden.plain(model)).items():
         g["init_sha256." + k] = np.array(v)
     g["param_order"] = np.array([k for k, _ in model.named_parameters()])
     import random

@@ -4,7 +4,7 @@ src/common/encoders.py):
     MMREC_REFERENCE_SRC=<MMRec checkout>/src python tests/golden/make_golden_selfcf.py
 
 Same harness and dataset (`tiny`) as make_golden_mvgae.py, `train_batch_size` 512.  Recorded:
-- the initial state as one SHA-256 per `state_dict` entry (selfcf_golden.init_digests);
+- the initial state as one SHA-256 per `state_dict` entry (golden_io.init_digests);
 - `sparse_norm_adj._indices()` and `_values()`: the stored entry order the encoder's dropout draws are applied in;
 - on one batch, in training mode and seeded (numpy and torch seed SEEDS["loss"]): the forward's `u_online`, `i_online`, the
   loss and every gradient, with the SHA-256 of each draw (selfcf_golden.Replay) and the rate;
@@ -30,6 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
 import selfcf_golden  # noqa: E402
@@ -41,7 +42,7 @@ TRAJ_SEED0 = 6000
 
 
 def _npz(g):
-    """`g`'s init digests as an in-memory npz (for `selfcf_golden.same_init`)."""
+    """`g`'s init digests as an in-memory npz (for `golden_io.same_init`)."""
     import io
     buf = io.BytesIO()
     np.savez(buf, **{k: v for k, v in g.items() if k.startswith("init_sha256.")})
@@ -111,7 +112,7 @@ def dump_selfcf(out):
     g["n_users"], g["n_items"] = np.int64(model.n_users), np.int64(model.n_items)
     for k in ("embedding_size", "n_layers", "dropout", "reg_weight", "train_batch_size", "learning_rate"):
         g["cfg_" + k] = np.float64(config[k])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g["init_sha256." + k] = np.array(v)
     g["param_order"] = np.array([k for k, _ in model.named_parameters()])
     adj = model.online_encoder.sparse_norm_adj
@@ -124,7 +125,7 @@ def dump_selfcf(out):
     g["batch"] = batch.numpy().copy()
     loss_phase(model, batch, "", g)
     _, _, _, _, model2 = make_golden.build("SELFCFED_LGN", dict(COMMON, n_layers=2))
-    assert model2.online_encoder.n_layers == 2 and not selfcf_golden.same_init(model2, np.load(_npz(g), allow_pickle=True))
+    assert model2.online_encoder.n_layers == 2 and not G.same_init(model2, np.load(_npz(g), allow_pickle=True))
     g["l2_cfg_n_layers"] = np.float64(2)
     loss_phase(model2, batch, "l2_", g)
 

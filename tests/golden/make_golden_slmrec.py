@@ -5,7 +5,7 @@
 Same harness and dataset (`tiny`) as make_golden_selfcf.py, `train_batch_size` 512, every grid key at its first value.
 `slmrec.py` imports `torch_scatter.scatter` at module top; the shim gets a stub of it (never called under FAC).  FAC draws
 nothing at random, so only the batching is seeded.  Recorded:
-- the initial state as one SHA-256 per `state_dict` entry (selfcf_golden.init_digests) and the parameter order;
+- the initial state as one SHA-256 per `state_dict` entry (golden_io.init_digests) and the parameter order;
 - `norm_adj._indices()` and `_values()` (`adj_type: pre`);
 - on one batch, in training mode: the three views `i_emb`, `v_emb`, `t_emb` of `compute()`, the loss and every gradient;
 - `full_sort_predict` on the first validation batch (the tables of that last `calculate_loss`) and the Trainer's
@@ -26,9 +26,9 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
-import selfcf_golden  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 COMMON = {"eval_batch_size": 128, "train_batch_size": 512}
@@ -45,7 +45,7 @@ def dump_slmrec(out):
     for k in ("recdim", "layer_num", "ssl_temp", "ssl_alpha", "temp", "learning_rate", "weight_decay", "train_batch_size"):
         g["cfg_" + k] = np.float64(config[k])
     g["cfg_adj_type"] = np.array(config["adj_type"])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g["init_sha256." + k] = np.array(v)
     g["param_order"] = np.array([k for k, _ in model.named_parameters()])
     g["adj_indices"] = model.norm_adj._indices().numpy().copy()

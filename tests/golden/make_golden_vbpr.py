@@ -5,7 +5,7 @@
 The unmodified model classes (`src/models/vbpr.py`, `src/models/bpr.py`) run under the harness, dataset and fields of
 make_golden.py (`tiny`, `train_batch_size` 512), with no shim.  vbpr_tiny.npz holds three VBPR cases under the prefixes of
 `CASES` (both modalities, text only, image only), bpr_tiny.npz one BPR case under "bpr.".  Per case, each tensor is kept as
-its SHA-256 and whole or as a fixed random sketch (dualgnn_golden.put):
+its SHA-256 and whole or as a fixed random sketch (golden_io.put):
 - the SHA-256 of every initial `state_dict` entry, the parameter order and the torch RNG state after construction;
 - one training batch, its [1]-shaped loss and every gradient;
 - `full_sort_predict` of the first validation batch, the trainer's top-50 of it (int16), and the validation and test
@@ -26,10 +26,9 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
+import golden_io as G  # noqa: E402
 import make_golden  # noqa: E402
 import ref_loader  # noqa: E402
-import selfcf_golden  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 COMMON = {"eval_batch_size": 128, "train_batch_size": 512}
@@ -47,7 +46,7 @@ def dump_model(g, prefix):
     p = prefix
     G.put_sha(g, p + "rng_after_init", torch.get_rng_state().numpy())
     g[p + "cfg"] = np.array([str(config["embedding_size"]), str(config["reg_weight"])])
-    for k, v in selfcf_golden.init_digests(model).items():
+    for k, v in G.init_digests(model).items():
         g[p + "init_sha256." + k] = np.array(v)
     g[p + "param_order"] = np.array([k for k, _ in model.named_parameters()])
 

@@ -29,7 +29,7 @@ def grad_errors(gold, grads: dict) -> dict:
     to ~1e-10 (the pos and neg rows carry opposite terms), pure reorder noise: they are measured against the scale of the
     other gradients, not their own."""
     import numpy as np
-    import dualgnn_golden as G
+    import golden_io as G
     pairs = {}
     for k, a in grads.items():
         a = np.asarray(a, dtype=np.float64)

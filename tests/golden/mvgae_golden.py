@@ -10,7 +10,7 @@ trajectory's eight batches.)"""
 import numpy as np
 import torch
 
-from lgmrec_golden import digest, pack  # noqa: F401  (re-exported for the generator)
+from golden_io import sha256_fp32
 
 
 def regenerate(gold, prefix):
@@ -25,28 +25,19 @@ def regenerate(gold, prefix):
             x = torch.empty(shape).bernoulli_(1 - p, generator=gen)
             x.div_(1 - p)
         a = x.numpy()
-        assert digest(a) == str(gold[prefix + "draw_sha256"][k]), f"{prefix}draw {k}: torch's CPU generator no longer gives the recorded draw"
+        assert sha256_fp32(a) == str(gold[prefix + "draw_sha256"][k]), f"{prefix}draw {k}: torch's CPU generator no longer gives the recorded draw"
         out.append(a)
     return out
 
 
-def init_digests(model) -> dict:
-    """SHA-256 of the fp32 bytes of every initial state: the `state_dict` entries (`param0.<name>`) and the plain tensors the
-    reference keeps beside its parameters (`plain.collaborative`, `plain.{v,t,c}_preference`, `plain.result_embed0`).  The
-    file keeps these digests, not the 1.2 MiB of incompressible weights: equal digests are equal bits."""
-    out = {"param0." + k: digest(v.detach().cpu().numpy()) for k, v in model.state_dict().items()}
-    out["plain.collaborative"] = digest(model.collaborative.detach().cpu().numpy())
+def plain(model) -> dict:
+    """The plain tensors the reference keeps beside its parameters, whose initial digests the files keep as
+    `init_sha256.plain.<name>` (`golden_io.init_digests`): not the 1.2 MiB of incompressible weights."""
+    out = {"collaborative": model.collaborative}
     for m in "vtc":
-        out["plain.%s_preference" % m] = digest(getattr(model, m + "_gcn").preference.detach().cpu().numpy())
-    out["plain.result_embed0"] = digest(model.result_embed.detach().cpu().numpy())
+        out["%s_preference" % m] = getattr(model, m + "_gcn").preference
+    out["result_embed0"] = model.result_embed
     return out
-
-
-def same_init(model, gold) -> list:
-    """Names of the initial states whose digest differs from the recorded one (empty: bit-identical), or whose set differs."""
-    want = {str(k)[len("init_sha256."):]: str(gold[k]) for k in gold.files if str(k).startswith("init_sha256.")}
-    got = init_digests(model)
-    return sorted(k for k in set(want) | set(got) if want.get(k) != got.get(k))
 
 
 def trajectory_draws(gold):

@@ -12,7 +12,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from lgmrec_golden import digest  # noqa: F401  (re-exported for the generator and the tests)
+from golden_io import sha256_fp32
 
 
 def cpu_dropout_mask(shape, p):
@@ -38,13 +38,13 @@ class Replay:
         if not training or p == 0 or input.numel() == 0:
             return input
         m = cpu_dropout_mask(tuple(input.shape), p)
-        self.digests.append(digest(m.numpy()))
+        self.digests.append(sha256_fp32(m.numpy()))
         return input * m.to(input.device)
 
     def rand(self, *size, **kw):
         x = self._rand(*size, **kw)
         if x.device.type == "cpu" and x.dtype == torch.float32:
-            self.digests.append(digest(x.numpy()))
+            self.digests.append(sha256_fp32(x.numpy()))
         return x
 
     def __enter__(self):
@@ -57,14 +57,3 @@ class Replay:
     def __exit__(self, *exc):
         F.dropout, torch.rand = self._saved
 
-
-def init_digests(model) -> dict:
-    """SHA-256 of the fp32 bytes of every `state_dict` entry (`param0.<name>`): equal digests are equal bits."""
-    return {"param0." + k: digest(v.detach().cpu().numpy()) for k, v in model.state_dict().items()}
-
-
-def same_init(model, gold) -> list:
-    """Names of the initial states whose digest differs from the recorded one (empty: bit-identical), or whose set differs."""
-    want = {str(k)[len("init_sha256."):]: str(gold[k]) for k in gold.files if str(k).startswith("init_sha256.")}
-    got = init_digests(model)
-    return sorted(k for k in set(want) | set(got) if want.get(k) != got.get(k))

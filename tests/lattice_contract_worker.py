@@ -1,31 +1,20 @@
-"""Worker of tests/test_lattice_contract.py (own process: the kernels behind `mmrec_b200.ops` are patched).
-
-LATTICE (`mmrec_b200.models.lattice`) under the harness of tests/dropin_contract_worker.py -- built the way quick_start
-builds it, the package's restatement or, with MMREC_REFERENCE_SRC, the reference's own code -- with the kernels replaced by
-`install_cpu_ops`'s CPU stand-ins plus torch restatements of the learned graph's operators (`ops.sddmm`,
+"""Worker of tests/test_lattice_contract.py: LATTICE (`mmrec_b200.models.lattice`) under the harness of tests/contract.py,
+with `install_cpu_ops`'s CPU stand-ins plus torch restatements of the learned graph's operators (`ops.sddmm`,
 `ops.csr_sym_norm`, `ops.spmm_values` and the pattern CSR the model builds directly), against tests/golden/lattice_tiny.npz
 and traj_lattice_tiny.npz recorded from the reference's class."""
 import copy
-import json
-import os
 import sys
-import tempfile
 
-import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.dirname(HERE))
-sys.path.insert(0, os.path.join(HERE, "golden"))
-sys.path.insert(0, HERE)
+import contract as C
+import golden_io as G
+from make_golden_lattice import CASES
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
-from dropin_contract_worker import CpuCSR, harness, install_cpu_ops  # noqa: E402
-from make_golden_lattice import CASES  # noqa: E402
+BATCHES = {"train_batch_size": 512}
 
 
-class LatticeCpuCSR(CpuCSR):
+class LatticeCpuCSR(C.CpuCSR):
     """`CpuCSR`, plus what LATTICE reads of `ops.CSR`: the constructor from (rowptr, colidx, vals), `vals` and
     `with_values`.  Entries are kept in CSR order (row, then stored column)."""
 
@@ -42,7 +31,7 @@ class LatticeCpuCSR(CpuCSR):
 
     @staticmethod
     def from_coo(*a, **k):
-        c = CpuCSR.from_coo(*a, **k)
+        c = C.CpuCSR.from_coo(*a, **k)
         return LatticeCpuCSR(c.t_, c.symmetric)
 
     def t(self):
@@ -55,7 +44,6 @@ class LatticeCpuCSR(CpuCSR):
 
 
 def install():
-    install_cpu_ops()
     from mmrec_b200 import graph, ops
     ops.CSR = graph.CSR = LatticeCpuCSR
     ops.sddmm = lambda A, P, Q: (P[A.row] * Q[A.col]).sum(1)
@@ -69,58 +57,13 @@ def install():
     ops.spmm_values = lambda A, vals, X: torch.zeros(A.n_rows, X.shape[1], dtype=X.dtype).index_add(0, A.row, vals.unsqueeze(1) * X[A.col])
 
 
-def _data(mods):
-    from mmrec_b200.utils import synth
-    tmp = tempfile.mkdtemp(prefix="mmrec_contract_")
-    data, *rest = harness(tmp)
-    u, i, e, d, f = synth.SHAPES["tiny"]
-    g = synth.make_graph(u, i, e, seed=0)
-    v, t = synth.make_features(i, f, seed=1)
-    synth.write_dataset(data, "tiny", g, v if "v" in mods else None, t if "t" in mods else None)
-    return rest
-
-
-def _build(rest, over, epochs=None):
-    Config, RecDataset, TrainDataLoader, EvalDataLoader, init_seed, Trainer, extra = rest
-    config = Config("LATTICE", "tiny", dict({"gpu_id": 0, "use_gpu": False, "train_batch_size": 512}, **over, **extra))
-    config["inter_file_name"] = "tiny.inter"
-    config["USER_ID_FIELD"], config["ITEM_ID_FIELD"] = "userID", "itemID"
-    config["vision_feature_file"], config["text_feature_file"] = "image_feat.npy", "text_feat.npy"
-    for k in config["hyper_parameters"]:
-        if isinstance(config[k], list):
-            config[k] = config[k][0]
-    if epochs:
-        config["epochs"] = epochs
-    dataset = RecDataset(config)
-    str(dataset)
-    tr, va, te = dataset.split()
-    str(tr), str(va), str(te)
-    train_data = TrainDataLoader(config, tr, batch_size=config["train_batch_size"], shuffle=True)
-    valid_data = EvalDataLoader(config, va, additional_dataset=tr, batch_size=config["eval_batch_size"])
-    test_data = EvalDataLoader(config, te, additional_dataset=tr, batch_size=config["eval_batch_size"])
-    init_seed(config["seed"])
-    train_data.pretrain_setup()
-    from mmrec_b200.models.lattice import LATTICE
-    model = LATTICE(config, train_data).to(config["device"])
-    return config, model, valid_data, test_data, Trainer
-
-
-def _sub(gold, p):
-    keys = [str(k) for k in gold.files]
-    if p:
-        return {k[len(p):]: gold[k] for k in keys if k.startswith(p)}
-    return {k: gold[k] for k in keys if not any(k.startswith(q) for q in CASES if q)}
-
-
-def check_case(rest, p, gold):
-    sub = _sub(gold, p)
-    config, model, valid_data, test_data, Trainer = _build(rest, dict(CASES[p][0]))
-    init = {k[len("init_sha256."):]: str(v) for k, v in sub.items() if k.startswith("init_sha256.")}
-    out = {"init_identical": selfcf_golden.init_digests(model) == init
-           and [k for k, _ in model.named_parameters()] == [str(x) for x in sub["param_order"]]}
+def check_case(p, gold):
+    over, mods = CASES[p]
+    h = C.build("LATTICE", mods, over=dict(over), batches=BATCHES, install=install)
+    model, sub = h.model, C.case(gold, p, CASES)
+    out = {"init_identical": C.check_init(model, sub)}
     model.train()
     model.pre_epoch_processing()
-    named = dict(model.named_parameters())
     out["grad_rel"], out["loss_rel"], out["grad_keys"] = 0.0, 0.0, True
     for tag in ("build.", "plain."):
         model.zero_grad(set_to_none=True)
@@ -128,61 +71,25 @@ def check_case(rest, p, gold):
         loss.backward()
         want = float(sub[tag + "loss"][0])
         out["loss_rel"] = max(out["loss_rel"], abs(float(loss.item()) - want) / abs(want))
-        grads = [k[len(tag + "grad."):] for k in G.recorded(sub, tag + "grad.")]
-        if tag == "plain." and not grads:                               # recorded for the first case only
+        if tag == "plain." and not G.recorded(sub, tag + "grad."):        # recorded for the first case only
             continue
-        out["grad_keys"] &= sorted(k for k, q in named.items() if q.grad is not None) == sorted(grads)
-        out["grad_rel"] = max([out["grad_rel"]] + [G.rel(sub, tag + "grad." + k, named[k].grad.numpy()) for k in grads])
+        keys_ok, rels = C.check_grads(model, sub, tag + "grad.")
+        out["grad_keys"] &= keys_ok
+        out["grad_rel"] = max([out["grad_rel"]] + list(rels.values()))
     model.zero_grad(set_to_none=True)
-    model.eval()
-    eb = [torch.from_numpy(sub["eval_users"]), torch.from_numpy(sub["eval_mask"])]
-    with torch.no_grad():
-        out["score_rel"] = G.rel(sub, "scores", model.full_sort_predict(eb).numpy())
-    trainer = Trainer(config, model)
-    valid = trainer.evaluate(valid_data)
-    test = trainer.evaluate(test_data, is_test=True)
-    names = [str(x) for x in sub["metric_names"]]
-    out["metric_max_abs"] = max(max(abs(valid[k] - w) for k, w in zip(names, sub["metric_values"])),
-                                max(abs(test[k] - w) for k, w in zip(names, sub["test_metric_values"])))
+    out["score_rel"] = G.rel(sub, "scores", C.predict(model, sub))
+    out.update(C.check_metrics(h, sub))
     return out
 
 
 def main_model():
-    gold = np.load(os.path.join(HERE, "golden", "lattice_tiny.npz"), allow_pickle=True)
-    install()
-    res = {}
-    for p, (_, mods) in CASES.items():
-        res[p or "default"] = check_case(_data(mods), p, gold)
-    print("CONTRACT " + json.dumps(res))
+    gold = C.load("lattice_tiny.npz")
+    C.emit({p or "default": check_case(p, gold) for p in CASES})
 
 
 def main_traj():
-    gold = np.load(os.path.join(HERE, "golden", "traj_lattice_tiny.npz"), allow_pickle=True)
-    install()
-    config, model, valid_data, test_data, Trainer = _build(_data("vt"), {}, epochs=2)
-    trainer = Trainer(config, model)
-    rec = {"losses": [], "valid": [], "test": []}
-    orig = model.calculate_loss
-
-    def spy(interaction):
-        l = orig(interaction)
-        rec["losses"].append(float(l.detach()))
-        return l
-    model.calculate_loss = spy
-    offs = np.concatenate([[0], np.cumsum(gold["batch_sizes"])])
-    first = np.concatenate([[0], np.cumsum(gold["batches_per_epoch"])])
-    recorded = [[torch.from_numpy(gold["batches"][:, offs[b]:offs[b + 1]].copy()) for b in range(first[ep], first[ep + 1])]
-                for ep in range(len(gold["batches_per_epoch"]))]
-    for ep in range(2):
-        model.pre_epoch_processing()
-        trainer._train_epoch(recorded[ep], ep)
-        trainer.lr_scheduler.step()
-        rec["valid"].append(list(trainer.evaluate(valid_data).values()))
-        rec["test"].append(list(trainer.evaluate(test_data, is_test=True).values()))
-    out = {"n_batches": len(rec["losses"]), "want_batches": int(gold["n_steps"]),
-           "loss_max_rel": float(np.max(np.abs(np.array(rec["losses"]) - gold["losses"]) / np.abs(gold["losses"]))),
-           "metric_max_abs": float(max(np.abs(np.array(rec["valid"]) - gold["valid"]).max(), np.abs(np.array(rec["test"]) - gold["test"]).max()))}
-    print("CONTRACT " + json.dumps(out))
+    h = C.build("LATTICE", batches=BATCHES, after={"epochs": 2}, install=install)
+    C.emit(C.replay_trajectory(h, C.load("traj_lattice_tiny.npz")))
 
 
 if __name__ == "__main__":

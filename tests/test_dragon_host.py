@@ -13,7 +13,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 
 CASES = {"": ({}, False), "text.": ({}, True), "mean.": ({"aggr_mode": ["mean"]}, False)}
 
@@ -82,7 +82,7 @@ def test_construction_order_and_state_dict_match_the_reference(cpu_graphs, data_
     model = _build(data_dirs[text_only], over)
     np_after, torch_after = np.random.randint(0, 2 ** 31, 4).astype(np.int64), torch.randint(0, 2 ** 31, (4,)).numpy()
     want = {str(k)[len(p + "init_sha256."):]: str(gold[k]) for k in gold.files if str(k).startswith(p + "init_sha256.")}
-    assert selfcf_golden.init_digests(model) == want                    # same keys in the same order, same bits
+    assert G.init_digests(model) == want                    # same keys in the same order, same bits
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold[p + "param_order"]]
     assert "result_embed" not in dict(model.named_parameters())
     assert model.result_embed.dtype == torch.float64 and model.result_embed.shape == (model.n_users + model.n_items, 64)

@@ -4,24 +4,11 @@ from the reference's class (tests/golden/make_golden_dualgnn.py), with the datas
 `synth.write_user_graph_dict`.
 
 Bit for bit: the initial weights and float64 `result_embed`, the float64 scores before any forward, the epoch's user-graph
-sample and the mutated batch.  Large tensors are compared through fixed random sketches (tests/golden/dualgnn_golden.py).
+sample and the mutated batch.  Large tensors are compared through fixed random sketches (tests/golden/golden_io.py).
 The propagation stand-in sums a row's neighbours in the coalesced sparse matrix's order and
 the user graph's duplicates are coalesced, where the reference scatters edge by edge and runs a batched matmul: towers,
 loss, gradients and scores agree to fp32 reorder error, and the metrics exactly."""
-import json
-import os
-import subprocess
-import sys
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _run(arg):
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "dualgnn_contract_worker.py"), arg], capture_output=True, text=True,
-                         timeout=900)
-    lines = [l for l in out.stdout.splitlines() if l.startswith("CONTRACT ")]
-    assert out.returncode == 0 and lines, out.stdout[-3000:] + out.stderr[-3000:]
-    return json.loads(lines[-1][len("CONTRACT "):])
+from contract import assert_metrics, run
 
 
 def _check_model(r):
@@ -31,20 +18,17 @@ def _check_model(r):
     assert abs(r["loss"] - r["want_loss"]) <= 1e-6 * abs(r["want_loss"])
     assert r["grad_keys"] and max(r["grad_rel"].values()) < 1e-5
     assert r["score_rel"] < 1e-5
-    for k, v in r["want_valid"].items():
-        assert abs(r["valid"][k] - v) < 1e-9, (k, r["valid"][k], v)
-    for k, v in r["want_test"].items():
-        assert abs(r["test"][k] - v) < 1e-9, (k, r["test"][k], v)
+    assert_metrics(r)
 
 
 def test_dualgnn_class_against_the_reference():
-    r = _run("model")
+    r = run("dualgnn_contract_worker.py", "model")
     assert r["has_v_gcn"] and set(r["rep_rel"]) == {"v_rep", "t_rep"}
     _check_model(r)
 
 
 def test_dualgnn_text_only_against_the_reference():
-    r = _run("text")
+    r = run("dualgnn_contract_worker.py", "text")
     assert not r["has_v_gcn"] and set(r["rep_rel"]) == {"t_rep"}
     _check_model(r)
 
@@ -52,6 +36,6 @@ def test_dualgnn_text_only_against_the_reference():
 def test_dualgnn_two_epoch_trajectory():
     """`Trainer._train_epoch` for two epochs on the recorded batches, `np.random` seeded before each epoch's sample: every
     batch loss and the per-epoch metrics."""
-    r = _run("traj")
+    r = run("dualgnn_contract_worker.py", "traj")
     assert r["n_batches"] == r["want_batches"] == 8
     assert r["loss_max_rel"] < 1e-5 and r["metric_max_abs"] < 1e-9

@@ -19,13 +19,14 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
-import dualgnn_golden as G  # noqa: E402
+import dualgnn_golden as D  # noqa: E402
+import golden_io as G  # noqa: E402
 from mmrec_b200 import graph  # noqa: E402
 from mmrec_b200.utils import synth  # noqa: E402
 
 
 def _graph(name):
-    return synth.named(name) if G.GRAPHS[name] is None else synth.make_graph(*G.GRAPHS[name])
+    return synth.named(name) if D.GRAPHS[name] is None else synth.make_graph(*D.GRAPHS[name])
 
 
 @functools.lru_cache(maxsize=None)
@@ -34,12 +35,12 @@ def _dict(name):
     return synth.user_graph_dict(_graph(name))
 
 
-@pytest.mark.parametrize("name", list(G.GRAPHS))
+@pytest.mark.parametrize("name", list(D.GRAPHS))
 def test_user_graph_dict_equals_the_script(golden, name):
     gold = golden("dualgnn_tiny.npz")
     path = synth.write_user_graph_dict(tempfile.mkdtemp(prefix="mmrec_ugd_"), name, _graph(name))
     d = np.load(path, allow_pickle=True).item()
-    ptr, idx, val = G.flatten(d)
+    ptr, idx, val = D.flatten(d)
     assert G.equal(gold, "ugd_%s_ptr" % name, ptr)
     assert G.equal(gold, "ugd_%s_idx" % name, idx)
     assert G.equal(gold, "ugd_%s_val" % name, val)
@@ -51,12 +52,12 @@ def test_user_graph_dict_equals_the_script(golden, name):
 
 def test_sampler_equals_the_reference(golden):
     gold = golden("dualgnn_tiny.npz")
-    np.random.seed(G.SAMPLE_SEED)
-    idx, w = graph.UserGraphTable(_dict("tiny"), G.K).sample(np.random)
+    np.random.seed(D.SAMPLE_SEED)
+    idx, w = graph.UserGraphTable(_dict("tiny"), D.K).sample(np.random)
     assert G.equal(gold, "sample_idx", idx) and G.equal(gold, "sample_w", w)
 
 
-@pytest.mark.parametrize("name", list(G.GRAPHS))
+@pytest.mark.parametrize("name", list(D.GRAPHS))
 @pytest.mark.parametrize("cut", [None, 7, 13])
 def test_vectorised_draws_and_softmax_equal_the_loop(name, cut):
     """One `randint` with an array of bounds draws what the reference's scalar calls draw, and the batched softmax gives
@@ -65,15 +66,15 @@ def test_vectorised_draws_and_softmax_equal_the_loop(name, cut):
     d = _dict(name)
     if cut:
         d = {u: [v[0][:(u * cut) % 60], v[1][:(u * cut) % 60]] for u, v in d.items()}
-    table = graph.UserGraphTable(d, G.K)
+    table = graph.UserGraphTable(d, D.K)
     if cut:
-        assert (table.n == 0).any() and ((table.n > 0) & (table.n < G.K)).sum() > 10
+        assert (table.n == 0).any() and ((table.n > 0) & (table.n < D.K)).sum() > 10
     for seed in (0, 11):
         np.random.seed(seed)
         a = table.sample(np.random)
         after_a = np.random.randint(0, 2 ** 31, 4)
         np.random.seed(seed)
-        b = G.topk_sample_loop(d, G.K)
+        b = D.topk_sample_loop(d, D.K)
         after_b = np.random.randint(0, 2 ** 31, 4)
         assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]) and np.array_equal(after_a, after_b)
     empty = table.n == 0

@@ -16,8 +16,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
+import dualgnn_golden as D  # noqa: E402
+import golden_io as G  # noqa: E402
 from make_golden_dragon import CASES  # noqa: E402
 from test_gpu_models import build  # noqa: E402
 
@@ -70,10 +70,10 @@ def test_dragon_matches_reference(envs, golden, p):
     config, train, valid, test, model = build("DRAGON", envs[CASES[p][1]], _overrides(p))
     dev = config["device"]
     init = {k[len("init_sha256."):]: str(v) for k, v in gold.items() if k.startswith("init_sha256.")}
-    assert selfcf_golden.init_digests(model) == init, "initial state differs from the reference"
+    assert G.init_digests(model) == init, "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold["param_order"]]
     assert "result_embed" not in dict(model.named_parameters())
-    assert G.sha256(model.result_embed.cpu().numpy()) == str(gold["result_embed0_sha256"])
+    assert G.sha256_tagged(model.result_embed.cpu().numpy()) == str(gold["result_embed0_sha256"])
     n_i = model.n_items
     mm = torch.zeros(n_i, n_i, dtype=torch.float64)
     mm[tuple(torch.from_numpy(gold["mm_adj_indices"]))] = torch.from_numpy(gold["mm_adj_values"]).double()
@@ -91,7 +91,7 @@ def test_dragon_matches_reference(envs, golden, p):
         m = s0.clone()
         m[eb[1][0], eb[1][1]] = -1e10
         assert torch.equal(idx0, torch.topk(m, 50, dim=-1)[1])
-    np.random.seed(G.SAMPLE_SEED)
+    np.random.seed(D.SAMPLE_SEED)
     model.pre_epoch_processing()
     assert G.equal(gold, "sample_idx", model.epoch_user_graph.numpy())
     assert G.equal(gold, "sample_w", model.user_weight_matrix.cpu().numpy())
@@ -172,7 +172,7 @@ def test_training_step_replayed_from_a_cuda_graph_gives_the_eager_bits(envs, gol
     gold = golden("dragon_tiny.npz")
     config, train, valid, test, model = build("DRAGON", envs[False], {})
     dev = config["device"]
-    np.random.seed(G.SAMPLE_SEED)
+    np.random.seed(D.SAMPLE_SEED)
     model.pre_epoch_processing()
     model.train()
     batch0 = torch.from_numpy(gold["batch"]).to(dev)

@@ -25,8 +25,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
+import dualgnn_golden as D  # noqa: E402
+import golden_io as G  # noqa: E402
 from test_gpu_models import build, rel  # noqa: E402
 
 EPS32 = 2.0 ** -24
@@ -128,7 +128,7 @@ def _sample(dev, seed=0):
     d = synth.user_graph_dict(synth.named("tiny"))
     d = {u: [v[0][:(u * 7) % 60], v[1][:(u * 7) % 60]] for u, v in d.items()}
     np.random.seed(seed)
-    return graph.UserGraphTable(d, G.K).sample(np.random)
+    return graph.UserGraphTable(d, D.K).sample(np.random)
 
 
 def _reference_aggregation(X, idx, w):
@@ -163,7 +163,7 @@ def test_user_graph_exact_operands_bit_for_bit(dev):
     w = (rng.integers(-4, 5, w.shape) * 0.125).astype(np.float32)
     w[empty] = 0.0
     w[~empty, 0] = 0.5                                                  # every other user keeps a non-zero row
-    assert empty.any() and any(len(set(r)) < G.K for r in idx[~empty])
+    assert empty.any() and any(len(set(r)) < D.K for r in idx[~empty])
     G_ = graph.build_user_graph(idx, w, dev)
     it, wt = torch.from_numpy(idx).to(dev), torch.from_numpy(w).to(dev)
     gen = torch.Generator().manual_seed(9)
@@ -175,7 +175,7 @@ def test_user_graph_exact_operands_bit_for_bit(dev):
     ref = _reference_aggregation(Xr, it, wt)
     ref.backward(up)
     M = torch.zeros(idx.shape[0], idx.shape[0], dtype=torch.float64, device=dev)
-    M.index_put_((torch.arange(idx.shape[0], device=dev).repeat_interleave(G.K), it.reshape(-1)), wt.reshape(-1).double(), accumulate=True)
+    M.index_put_((torch.arange(idx.shape[0], device=dev).repeat_interleave(D.K), it.reshape(-1)), wt.reshape(-1).double(), accumulate=True)
     assert torch.equal(out.detach().double(), X.detach().double() + M @ X.detach().double())
     assert torch.equal(X.grad.double(), up.double() + M.t() @ up.double())
     assert torch.equal(out.detach(), ref.detach()) and torch.equal(X.grad, Xr.grad)
@@ -186,7 +186,7 @@ def test_user_graph_memory_at_clothing_shape(dev):
     fp32 tensor (410 MB) and keeps it for the backward.  The op's peak allocation above what was allocated before it, over
     the forward and the backward, must stay below an eighth of that.  The CSR and its transpose are built first."""
     from mmrec_b200 import graph, ops
-    U, k, d = 40000, G.K, 64
+    U, k, d = 40000, D.K, 64
     rng = np.random.default_rng(0)
     idx = rng.integers(0, U, (U, k)).astype(np.int64)
     short = rng.random(U) < 0.2
@@ -244,11 +244,11 @@ def test_dualgnn_matches_reference(env, env_text, golden, p):
     config, train, valid, test, model = build("DualGNN", env_text if p else env, {})
     dev = config["device"]
     init = {k[len("init_sha256.param0."):]: str(v) for k, v in gold.items() if k.startswith("init_sha256.")}
-    got = {k[len("param0."):]: v for k, v in selfcf_golden.init_digests(model).items()}
+    got = {k[len("param0."):]: v for k, v in G.init_digests(model).items()}
     assert got == init, "initial state differs from the reference"       # same keys: a reference state_dict loads strictly
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold["param_order"]]
     assert "result_embed" not in dict(model.named_parameters())
-    assert G.sha256(model.result_embed.cpu().numpy()) == str(gold["result_embed0_sha256"])
+    assert G.sha256_tagged(model.result_embed.cpu().numpy()) == str(gold["result_embed0_sha256"])
     eb = [torch.from_numpy(gold["eval_users"]).to(dev), torch.from_numpy(gold["eval_mask"]).to(dev)]
     model.eval()
     with torch.no_grad():
@@ -260,7 +260,7 @@ def test_dualgnn_matches_reference(env, env_text, golden, p):
         m = s0.clone()
         m[eb[1][0], eb[1][1]] = -1e10
         assert torch.equal(idx0, torch.topk(m, 50, dim=-1)[1])
-    np.random.seed(G.SAMPLE_SEED)
+    np.random.seed(D.SAMPLE_SEED)
     model.pre_epoch_processing()
     assert G.equal(gold, "sample_idx", model.epoch_user_graph.numpy())
     assert G.equal(gold, "sample_w", model.user_weight_matrix.cpu().numpy())

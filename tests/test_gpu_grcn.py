@@ -20,8 +20,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 from make_golden_grcn import CASES, TRAJ_LR, MessagePassing, softmax  # noqa: E402
 from test_gpu_models import build  # noqa: E402
 
@@ -343,7 +342,7 @@ def test_grcn_matches_reference(envs, golden, p):
     config, train, valid, test, model = build("GRCN", envs[CASES[p][1]], dict(CASES[p][0]))
     dev = config["device"]
     init = {k[len("init_sha256."):]: str(v) for k, v in gold.items() if k.startswith("init_sha256.")}
-    assert selfcf_golden.init_digests(model) == init, "initial state differs from the reference"
+    assert G.init_digests(model) == init, "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold["param_order"]]
     eb = [torch.from_numpy(gold["eval_users"]).to(dev), torch.from_numpy(gold["eval_mask"]).to(dev)]
     model.eval()

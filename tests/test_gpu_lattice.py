@@ -17,8 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 from make_golden_lattice import CASES  # noqa: E402
 from test_gpu_models import build  # noqa: E402
 
@@ -244,7 +243,7 @@ def test_lattice_matches_reference(envs, golden, p):
     n = model.n_items
     graph_key = p + "item_adj" if p + "item_adj.index" in full.files else "item_adj"   # recorded where it differs from the first case's
     init = {k[len("init_sha256."):]: str(v) for k, v in gold.items() if k.startswith("init_sha256.")}
-    assert selfcf_golden.init_digests(model) == init, "initial state differs from the reference"
+    assert G.init_digests(model) == init, "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold["param_order"]]
     r, c, v = model.norm_adj.coo()
     assert np.array_equal(np.stack([r.cpu().numpy(), c.cpu().numpy()]), full["norm_adj_indices"])

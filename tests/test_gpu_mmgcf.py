@@ -26,9 +26,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
+import golden_io as G  # noqa: E402
 import mmgcf_golden as M  # noqa: E402
-import selfcf_golden  # noqa: E402
 from test_gpu_models import build  # noqa: E402
 
 MODES = [(f, w) for f in ("mean", "sum") for w in ("equal", "alpha", "normalized")]
@@ -155,7 +154,7 @@ def test_mmgcf_matches_reference(envs, golden, name):
     config, train, valid, test, model = build("MMGCF", envs[text_only], M.overrides(fusion, weighting, layers))
     dev = config["device"]
     init = {k[len("init_sha256."):]: str(v) for k, v in sub.items() if k.startswith("init_sha256.")}
-    assert selfcf_golden.init_digests(model) == init, "initial state differs from the reference"
+    assert G.init_digests(model) == init, "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in sub["param_order"]]
     assert G.equal(gold, "edge_values", model.edge_values.cpu().numpy())
     model.masked_adj = model.pruner.adj_from_keep(torch.from_numpy(gold["prune_keep_idx"]).to(dev))

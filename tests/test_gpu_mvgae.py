@@ -193,6 +193,7 @@ def test_max_dot_memory_at_8192():
 # the model class against the reference's golden files
 # ------------------------------------------------------------------------------------------------
 sys.path.insert(0, os.path.join(HERE, "golden"))
+import golden_io as G  # noqa: E402
 import mvgae_golden  # noqa: E402
 from test_gpu_models import build, check_topk, rel  # noqa: E402
 
@@ -248,7 +249,7 @@ def test_mvgae_matches_reference(env, golden, monkeypatch):
     gold = golden("mvgae_tiny.npz")
     config, train, valid, test, model = build("MVGAE", env, {})
     dev = config["device"]
-    assert mvgae_golden.same_init(model, gold) == [], "initial state differs from the reference"
+    assert G.same_init(model, gold, mvgae_golden.plain(model)) == [], "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == list(gold["param_order"])
     model.eval()
     with Replay([], dev), torch.no_grad():

@@ -252,6 +252,7 @@ def test_unsupported_width_is_an_error(dev):
 # ----------------------------------------------------------------------------------------------------------------------
 # the model class against the reference's golden files
 # ----------------------------------------------------------------------------------------------------------------------
+import golden_io as G  # noqa: E402
 import selfcf_golden  # noqa: E402
 from test_gpu_models import build, check_topk, rel  # noqa: E402
 
@@ -274,7 +275,7 @@ def test_selfcf_matches_reference(env, golden):
     gold = golden("selfcfed_lgn_tiny.npz")
     config, train, valid, test, model = build("SELFCFED_LGN", env, {})
     dev = config["device"]
-    assert selfcf_golden.same_init(model, gold) == [], "initial state differs from the reference"
+    assert G.same_init(model, gold) == [], "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == list(gold["param_order"])
     enc = model.online_encoder
     r, c, v = enc.sparse_norm_adj.coo()

@@ -14,6 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, HERE)
 
+import golden_io as G  # noqa: E402
 import selfcf_golden  # noqa: E402
 from test_gpu_models import build, rel  # noqa: E402
 
@@ -37,7 +38,7 @@ def test_selfcf_two_layers_match_reference(env, golden):
     config, train, valid, test, model = build("SELFCFED_LGN", env, {"n_layers": 2})
     dev = config["device"]
     assert model.online_encoder.n_layers == 2
-    assert selfcf_golden.same_init(model, gold) == [], "initial state differs from the reference"
+    assert G.same_init(model, gold) == [], "initial state differs from the reference"
     model.train()
     model.zero_grad()
     fwd = []

@@ -139,7 +139,7 @@ def test_gate_at_width_3d(dev, d):
 # ----------------------------------------------------------------------------------------------------------------------
 # the model class against the reference's golden files
 # ----------------------------------------------------------------------------------------------------------------------
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 from test_gpu_models import build, rel  # noqa: E402
 
 
@@ -162,7 +162,7 @@ def test_slmrec_matches_reference(env, golden):
     gold = golden("slmrec_tiny.npz")
     config, train, valid, test, model = build("SLMRec", env, {})
     dev = config["device"]
-    assert selfcf_golden.same_init(model, gold) == [], "initial state differs from the reference"
+    assert G.same_init(model, gold) == [], "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == list(gold["param_order"])
     assert model.norm_adj.symmetric
     r, c, v = model.norm_adj.coo()

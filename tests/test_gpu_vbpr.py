@@ -20,8 +20,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, HERE)
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 import vbpr_golden as V  # noqa: E402
 from test_gpu_models import build  # noqa: E402
 
@@ -280,7 +279,7 @@ def test_model_matches_reference(envs, golden, p):
     config, train, valid, test, model = build(name, envs[mods], {})
     dev = config["device"]
     init = {k[len("init_sha256."):]: str(v) for k, v in gold.items() if k.startswith("init_sha256.")}
-    assert selfcf_golden.init_digests(model) == init, "initial state differs from the reference"
+    assert G.init_digests(model) == init, "initial state differs from the reference"
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold["param_order"]]
     model.train()
     model.zero_grad(set_to_none=True)

@@ -15,7 +15,7 @@ import torch.nn.functional as F
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 from make_golden_grcn import CASES, MessagePassing, softmax  # noqa: E402
 
 
@@ -74,13 +74,12 @@ def test_config_takes_the_reference_keys_and_values(data_dirs, gold):
 
 @pytest.mark.parametrize("p", list(CASES))
 def test_construction_order_and_rng_consumption_match_the_reference(cpu_graphs, data_dirs, gold, p):
-    import dualgnn_golden as G
     over, mods = CASES[p]
     model, _ = _build(data_dirs[mods], dict(over))
     assert G.equal(gold, p + "rng_after_init", torch.get_rng_state().numpy())
     want = {str(k)[len(p + "init_sha256."):]: str(gold[k]) for k in gold.files
             if str(k).startswith(p + "init_sha256.") and (p or not any(str(k).startswith(q) for q in CASES if q))}
-    assert selfcf_golden.init_digests(model) == want
+    assert G.init_digests(model) == want
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold[p + "param_order"]]
     assert "v_gcn.features" not in model.state_dict() and model.result.shape == (model.n_users + model.n_items, 64)
 

@@ -2,9 +2,7 @@
 reference's class (tests/golden/make_golden_itemknncbf.py); the class under the quick_start-built harness with CPU stand-ins
 for K7's shrink route and K9; K9's ranking rule against a dense ranking on crafted rows; the argument errors of the new
 entry points."""
-import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -15,6 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import itemknncbf_oracle as KO  # noqa: E402
+from contract import assert_metrics, run  # noqa: E402
 
 PREFIXES = ["s10_", "s0_"]
 
@@ -53,26 +52,15 @@ def test_oracle_equals_the_reference(gold, prefix):
     assert np.array_equal(sm[G("eval_users")].view(np.uint32), G("scores").view(np.uint32))
 
 
-def _run(prefix):
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "itemknncbf_contract_worker.py"), prefix], capture_output=True,
-                         text=True, timeout=900)
-    lines = [l for l in out.stdout.splitlines() if l.startswith("CONTRACT ")]
-    assert out.returncode == 0 and lines, out.stdout[-3000:] + out.stderr[-3000:]
-    return json.loads(lines[-1][len("CONTRACT "):])
-
-
 @pytest.mark.parametrize("prefix", PREFIXES)
 def test_itemknncbf_class_against_the_reference(prefix):
     """The kNN graph (the stand-in evaluates the similarity in float64: the recorded neighbours except near ties, values
     within the fp32 bound), the predictions to 1e-6 relative, the one parameter, and the valid / test metrics of
     `Trainer.evaluate`."""
-    r = _run(prefix)
+    r = run("itemknncbf_contract_worker.py", prefix)
     assert r["knn_ok"] and r["dummy_ok"] and r["params"] == ["dummy_embeddings"]
     assert r["score_err"] < 1e-6
-    for k, v in r["want_valid"].items():
-        assert abs(r["valid"][k] - v) < 1e-9, (k, r["valid"][k], v)
-    for k, v in r["want_test"].items():
-        assert abs(r["test"][k] - v) < 1e-9, (k, r["test"][k], v)
+    assert_metrics(r)
 
 
 def _crafted_rows():

@@ -15,7 +15,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 from make_golden_lattice import CASES  # noqa: E402
 
 
@@ -84,7 +84,7 @@ def test_construction_order_and_initial_state_match_the_reference(cpu_graphs, da
     model, _ = _build(data_dirs[mods], dict(over))
     want = {str(k)[len(p + "init_sha256."):]: str(gold[k]) for k in gold.files
             if str(k).startswith(p + "init_sha256.") and (p or not any(str(k).startswith(q) for q in CASES if q))}
-    assert selfcf_golden.init_digests(model) == want
+    assert G.init_digests(model) == want
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold[p + "param_order"]]
 
 

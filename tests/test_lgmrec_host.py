@@ -2,42 +2,28 @@
 MMREC_REFERENCE_SRC, else the package's restatement), kernels replaced by CPU stand-ins, against the golden files recorded from
 the reference's class (tests/golden/make_golden_lgmrec.py) under the reference's own RNG stream; and the argument errors of
 K8's entry points (include/mmrec_b200.h)."""
-import json
 import os
-import subprocess
-import sys
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _run(arg):
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "lgmrec_contract_worker.py"), arg], capture_output=True, text=True,
-                         timeout=900)
-    lines = [l for l in out.stdout.splitlines() if l.startswith("CONTRACT ")]
-    assert out.returncode == 0 and lines, out.stdout[-3000:] + out.stderr[-3000:]
-    return json.loads(lines[-1][len("CONTRACT "):])
+from contract import assert_metrics, run
 
 
 @pytest.mark.parametrize("gfile", ["lgmrec_tiny.npz", "lgmrec_clothing_tiny.npz"])
 def test_lgmrec_class_against_the_reference(gfile):
     """Initial weights bit for bit and in the reference's parameter order, `num_inters`, the same Gumbel / dropout draws in
     every phase, forward, loss, gradients, first-batch scores and the valid / test metrics of `Trainer.evaluate`."""
-    r = _run(gfile)
+    r = run("lgmrec_contract_worker.py", gfile)
     assert r["init_identical"] and r["graphs"] and r["draws_ok"]
     assert r["fwd_rel"] < 1e-6 and r["grad_rel"] < 1e-5 and r["score_err"] < 1e-6
     assert abs(r["loss"] - r["want_loss"]) <= 1e-6 * abs(r["want_loss"])
-    for k, v in r["want_valid"].items():
-        assert abs(r["valid"][k] - v) < 1e-9, (k, r["valid"][k], v)
-    for k, v in r["want_test"].items():
-        assert abs(r["test"][k] - v) < 1e-9, (k, r["test"][k], v)
+    assert_metrics(r)
 
 
 def test_lgmrec_two_epoch_trajectory():
     """`Trainer._train_epoch` for two epochs on the recorded batches and draws: every batch loss and the per-epoch metrics."""
-    r = _run("traj")
+    r = run("lgmrec_contract_worker.py", "traj")
     assert r["n_batches"] == 8 and r["draws_left"] == 0
     assert r["loss_max_rel"] < 1e-6 and r["metric_max_abs"] < 1e-9
 

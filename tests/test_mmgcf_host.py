@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
 import mmgcf_golden as M  # noqa: E402
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 
 
 class _Pruner:
@@ -66,7 +66,7 @@ def test_construction_order_and_state_dict_match_the_reference(cpu_graphs, data_
     fusion, weighting, layers, text_only = M.CASES[name]
     model = _build(data_dirs[text_only], M.overrides(fusion, weighting, layers))
     want = {str(k)[len(name) + len(".init_sha256."):]: str(gold[k]) for k in gold.files if str(k).startswith(name + ".init_sha256.")}
-    assert selfcf_golden.init_digests(model) == want                    # same keys in the same order, same bits
+    assert G.init_digests(model) == want                    # same keys in the same order, same bits
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold[name + ".param_order"]]
     assert not model.image_embedding.weight.requires_grad if not text_only else not hasattr(model, "image_embedding")
     assert not model.text_embedding.weight.requires_grad

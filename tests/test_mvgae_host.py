@@ -1,46 +1,32 @@
 """MVGAE without a GPU: the class under the harness the reference's quick_start builds (its own code with
 MMREC_REFERENCE_SRC, else the package's restatement), kernels replaced by CPU stand-ins, against the golden files recorded from
 the reference's class (tests/golden/make_golden_mvgae.py) under the reference's own RNG stream."""
-import json
 import os
-import subprocess
-import sys
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _run(arg):
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mvgae_contract_worker.py"), arg], capture_output=True, text=True,
-                         timeout=900)
-    lines = [l for l in out.stdout.splitlines() if l.startswith("CONTRACT ")]
-    assert out.returncode == 0 and lines, out.stdout[-3000:] + out.stderr[-3000:]
-    return json.loads(lines[-1][len("CONTRACT "):])
+from contract import assert_metrics, run
 
 
 def test_mvgae_class_against_the_reference():
     """Initial weights and plain tensors bit for bit (their SHA-256), in the reference's parameter order; the same dropout masks and Gaussian
     noise; forward, the four decodes (values, and the argmax except at near ties), loss, gradients of every Parameter that
     gets one, first-batch scores of the cached `result_embed`, and the valid / test metrics of `Trainer.evaluate`."""
-    r = _run("model")
+    r = run("mvgae_contract_worker.py", "model")
     assert r["init_identical"] and r["draws_ok"]
     assert r["fwd_rel"] < 1e-6
     assert r["n_decodes"] == 4 and r["decode_rel"] < 1e-6 and r["argmax_near_ties"]
     assert abs(r["loss"] - r["want_loss"]) <= 1e-6 * abs(r["want_loss"])
     assert r["grad_keys"] and r["grad_rel"] < 1e-5
     assert r["score_err"] < 1e-6
-    for k, v in r["want_valid"].items():
-        assert abs(r["valid"][k] - v) < 1e-9, (k, r["valid"][k], v)
-    for k, v in r["want_test"].items():
-        assert abs(r["test"][k] - v) < 1e-9, (k, r["test"][k], v)
+    assert_metrics(r)
 
 
 def test_mvgae_two_epoch_trajectory():
     """`Trainer._train_epoch` for two epochs on the recorded batches and draws: every batch loss and the per-epoch metrics
     (scored from the last training forward's `result_embed`, as the reference does)."""
-    r = _run("traj")
+    r = run("mvgae_contract_worker.py", "traj")
     assert r["n_batches"] == 8 and r["draws_left"] == 0
     assert r["loss_max_rel"] < 1e-6 and r["metric_max_abs"] < 1e-9
 

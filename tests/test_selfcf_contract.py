@@ -2,20 +2,7 @@
 builds (its own code with MMREC_REFERENCE_SRC, else the package's restatement), kernels replaced by CPU stand-ins, against the
 golden files recorded from the reference's class (tests/golden/make_golden_selfcf.py).  The class draws the rate, the edge
 dropout and the target masks itself from the seeded CPU generators; the draws are compared by digest."""
-import json
-import os
-import subprocess
-import sys
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _run(arg):
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "selfcf_contract_worker.py"), arg], capture_output=True, text=True,
-                         timeout=900)
-    lines = [l for l in out.stdout.splitlines() if l.startswith("CONTRACT ")]
-    assert out.returncode == 0 and lines, out.stdout[-3000:] + out.stderr[-3000:]
-    return json.loads(lines[-1][len("CONTRACT "):])
+from contract import assert_metrics, run
 
 
 def _check_loss_phase(r, n_layers):
@@ -31,23 +18,20 @@ def test_selfcf_class_against_the_reference():
     """Initial weights bit for bit (their SHA-256) in the reference's parameter order; the same draws; forward rows, loss and
     gradients; first-batch scores (one width-2d product against the reference's two products and an add: fp32 reorder
     error); the valid / test metrics of `Trainer.evaluate`."""
-    r = _run("model")
+    r = run("selfcf_contract_worker.py", "model")
     _check_loss_phase(r, 1)
     assert r["score_err"] < 1e-5
-    for k, v in r["want_valid"].items():
-        assert abs(r["valid"][k] - v) < 1e-9, (k, r["valid"][k], v)
-    for k, v in r["want_test"].items():
-        assert abs(r["test"][k] - v) < 1e-9, (k, r["test"][k], v)
+    assert_metrics(r)
 
 
 def test_selfcf_two_layers_against_the_reference():
     """The class built with `n_layers` = 2: two dropped layers forward and the backward through both."""
-    _check_loss_phase(_run("layers2"), 2)
+    _check_loss_phase(run("selfcf_contract_worker.py", "layers2"), 2)
 
 
 def test_selfcf_two_epoch_trajectory():
     """`Trainer._train_epoch` for two epochs on the recorded batches, each seeded as recorded: every batch's draws and loss,
     and the per-epoch metrics."""
-    r = _run("traj")
+    r = run("selfcf_contract_worker.py", "traj")
     assert r["n_batches"] == r["want_batches"] == 8 and r["draws_ok"]
     assert r["loss_max_rel"] < 1e-6 and r["metric_max_abs"] < 1e-9

@@ -13,6 +13,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
+import golden_io as G  # noqa: E402
 from mmrec_b200 import graph  # noqa: E402
 
 
@@ -102,10 +103,10 @@ def test_golden_draws_regenerate(golden):
     rep = selfcf_golden.Replay(gold["loss_seed"])
     rep.seed_phase()
     assert np.random.random() == float(gold["loss_rate"])
-    digests = [selfcf_golden.digest(torch.rand(nnz).numpy())]
+    digests = [G.sha256_fp32(torch.rand(nnz).numpy())]
     B = gold["batch"].shape[1]
     for _ in range(2):
-        digests.append(selfcf_golden.digest(selfcf_golden.cpu_dropout_mask((B, int(gold["cfg_embedding_size"])), float(gold["cfg_dropout"])).numpy()))
+        digests.append(G.sha256_fp32(selfcf_golden.cpu_dropout_mask((B, int(gold["cfg_embedding_size"])), float(gold["cfg_dropout"])).numpy()))
     assert digests == list(gold["loss_draw_sha256"])
 
 
@@ -124,9 +125,9 @@ def test_dropped_propagation_oracle_matches_the_reference_forward(golden):
     d = int(gold["cfg_embedding_size"])
     ue = torch.nn.init.xavier_uniform_(torch.empty(nu, d))
     ie = torch.nn.init.xavier_uniform_(torch.empty(ni, d))
-    if selfcf_golden.digest(ue.numpy()) != str(gold["init_sha256.param0.online_encoder.embedding_dict.user_emb"]):
+    if G.sha256_fp32(ue.numpy()) != str(gold["init_sha256.param0.online_encoder.embedding_dict.user_emb"]):
         pytest.skip("the harness seeds differently from init_seed(999) + manual_seed here")
-    assert selfcf_golden.digest(ie.numpy()) == str(gold["init_sha256.param0.online_encoder.embedding_dict.item_emb"])
+    assert G.sha256_fp32(ie.numpy()) == str(gold["init_sha256.param0.online_encoder.embedding_dict.item_emb"])
     rep = selfcf_golden.Replay(gold["loss_seed"])
     rep.seed_phase()
     rate = np.random.random()

@@ -12,8 +12,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
-import dualgnn_golden as G  # noqa: E402
-import selfcf_golden  # noqa: E402
+import golden_io as G  # noqa: E402
 import vbpr_golden as V  # noqa: E402
 
 
@@ -66,7 +65,7 @@ def test_construction_order_and_rng_consumption_match_the_reference(data_dirs, g
     model, config = _build(name, data_dirs[mods])
     assert G.equal(gold, p + "rng_after_init", torch.get_rng_state().numpy())
     want = {str(k)[len(p + "init_sha256."):]: str(gold[k]) for k in gold.files if str(k).startswith(p + "init_sha256.")}
-    assert selfcf_golden.init_digests(model) == want                    # same keys in the same order, same bits
+    assert G.init_digests(model) == want                    # same keys in the same order, same bits
     assert [k for k, _ in model.named_parameters()] == [str(x) for x in gold[p + "param_order"]]
     assert list(gold[p + "cfg"]) == [str(config["embedding_size"]), str(config["reg_weight"])]
     if name == "VBPR":
