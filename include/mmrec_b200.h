@@ -589,6 +589,43 @@ int mmrec_bpr_mf_bwd_f32(int64_t B, int du, int da, int dp, const float* U, cons
                          const int64_t* pos, const int64_t* neg, float reg_weight, const float* x, const float* norms,
                          const float* g, float* gU, float* gA_rows, float* gP_rows, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * n14  PGL's loss after the tables (src/models/pgl.py:227-259): `bpr_loss` (-mean(logsigmoid(<u,p> - <u,n>))) plus
+ * reg_weight * (InfoNCE(a, b) + InfoNCE(c, d)) / 2, the views a, b (c, d) two dropout draws of the user (positive item)
+ * rows, InfoNCE(v, w) = mean_b -log(exp(<v^_b, w^_b> / 0.2) / sum_j exp(<v^_b, w^_j> / 0.2)), v^ = F.normalize(v).
+ * The B x B sums are K8's (mmrec_expsum_rows_f32 / _bwd_f32, inv_tau 5) on the views the row call writes; the caller runs them
+ * between the calls below (ops.pgl_loss).
+ *   UA [n_users, d], IA [n_items, d]; users / pos / neg int64 [B], may repeat, entries in range (not checked).  m0..m3: the
+ *   dropout's bool masks [B, d] of a, b, c, d (uint8 0 / 1), all four or none (none: keep every entry); a view is
+ *   (row * m) * scale, ATen's fused dropout with scale = fp32(1 / fp32(1 - p)).
+ *   mmrec_pgl_rows_f32:      x[b] = <u_b, p_b> - <u_b, n_b>; with va..vd, vnorm [4, B] and pd [2, B] (all or none) also the
+ *                            normalised views, their norms before clamp_min, and pd = (<a^_b, b^_b>, <c^_b, d^_b>).
+ *   mmrec_pgl_finish_f32:    the 0-dim loss from x and, with pd, ttl1 = K8(a^, b^) and ttl2 = K8(c^, d^) (all or none; none:
+ *                            reg_weight * cl is taken as an exact 0, valid while every input is finite).
+ *   mmrec_pgl_finish_bwd_f32: for the upstream gradient g (one fp32, read on the device): gx [B], and with pd / ttl gpd [2, B]
+ *                            (the positive dots' gradients) and gttl [2, B] (K8's upstream gradients).
+ *   mmrec_pgl_rows_bwd_f32:  gU [B, d] (scatter by users) and gI [2B, d] ([pos rows; neg rows]) from gx and, all or none,
+ *                            vnorm, gpd and gva..gvd (K8's gradients of the views); scale_bwd is the dropout backward's
+ *                            fp32(1 / (1 - p)).
+ *   Rounding: every element-wise step is torch's on the device, one IEEE fp32 rounding each, the divisions by Python numbers
+ *   as multiplications by their fp32 reciprocals, a row's gradients added in autograd's order (the InfoNCE views, then the
+ *   negative and the positive BPR term).  Dots, sums of squares and the normaliser's row sums run in the kernel's own fixed
+ *   order; the batch sums are one CTA's in a fixed order: the same bits on every run.  No host synchronisation.
+ *  - One warp per row; d a multiple of 128 (64) with aligned operands is vectorised, any d >= 1 is correct.
+ *  - B < 1, d < 1, a null pointer or an incomplete optional group return MMREC_EINVAL before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+int mmrec_pgl_rows_f32(int64_t B, int d, const float* UA, const float* IA, const int64_t* users, const int64_t* pos,
+                       const int64_t* neg, const uint8_t* m0, const uint8_t* m1, const uint8_t* m2, const uint8_t* m3, float scale,
+                       float* x, float* va, float* vb, float* vc, float* vd, float* vnorm, float* pd, void* stream);
+int mmrec_pgl_finish_f32(int64_t B, const float* x, const float* pd, const float* ttl1, const float* ttl2, float reg_weight,
+                         float* loss, void* stream);
+int mmrec_pgl_finish_bwd_f32(int64_t B, const float* x, const float* pd, const float* ttl1, const float* ttl2, float reg_weight,
+                             const float* g, float* gx, float* gpd, float* gttl, void* stream);
+int mmrec_pgl_rows_bwd_f32(int64_t B, int d, const float* UA, const float* IA, const int64_t* users, const int64_t* pos,
+                           const int64_t* neg, const uint8_t* m0, const uint8_t* m1, const uint8_t* m2, const uint8_t* m3,
+                           float scale_bwd, float scale, const float* gx, const float* vnorm, const float* gpd, const float* gva,
+                           const float* gvb, const float* gvc, const float* gvd, float* gU, float* gI, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -86,6 +86,11 @@ PROTOTYPES = {
     "mmrec_bpr_mf_workspace_bytes": (_sz, [_i64]),
     "mmrec_bpr_mf_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _f32, _p, _p, _p, _p, _sz, _p]),
     "mmrec_bpr_mf_bwd_f32": (_i32, [_i64, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _f32, _p, _p, _p, _p, _p, _p, _p]),
+    "mmrec_pgl_rows_f32": (_i32, [_i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _f32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "mmrec_pgl_finish_f32": (_i32, [_i64, _p, _p, _p, _p, _f32, _p, _p]),
+    "mmrec_pgl_finish_bwd_f32": (_i32, [_i64, _p, _p, _p, _p, _f32, _p, _p, _p, _p, _p]),
+    "mmrec_pgl_rows_bwd_f32": (_i32, [_i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _f32, _f32, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                                      _p]),
 }
 
 class SpmmOp(C.Structure):

@@ -347,8 +347,11 @@ class EdgePruner:
         return CSR.from_coo(torch.cat((u, iu)), torch.cat((iu, u)), torch.cat((vals, vals)), n, n,
                             sum_duplicates=True, symmetric=True)
 
-    def sample(self, dropout: float):
-        keep_len = int(self.edge_values.size(0) * (1.0 - dropout))
+    def sample(self, dropout: Optional[float] = None, keep_len: Optional[int] = None):
+        """The epoch's pruned graph and the kept edges: `keep_len` edges (default `int(nnz * (1 - dropout))`, FREEDOM's;
+        PGL's `int(nnz * 0.3)` is given as is, as the float product can round differently) drawn without replacement."""
+        if keep_len is None:
+            keep_len = int(self.edge_values.size(0) * (1.0 - dropout))
         keep_idx = torch.multinomial(self.edge_values, keep_len)
         return self.adj_from_keep(keep_idx), keep_idx
 

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import copy
 import ctypes
-from typing import Optional
+from typing import Optional, Sequence
 
 import torch
 
@@ -1096,6 +1096,129 @@ def bpr_mf_loss(U: torch.Tensor, A: torch.Tensor, P: Optional[torch.Tensor], use
     gradients equal its bits; the batch sums are the same bits on every run.  Never synchronises with the host."""
     U, A, P, (users, pos, neg), B, du, da, dp = _bpr_mf_args(U, A, P, users, pos, neg)
     return _BprMfFn.apply(U, A, P, users, pos, neg, float(reg_weight))
+
+
+# -- n14: PGL's BPR + self-contrastive loss (csrc/pgl_loss.cu, with K8 for the B x B sums) -------------------------------
+PGL_TAU = 0.2                                               # InfoNCE's temperature (src/models/pgl.py:255-256)
+
+
+def dropout_scales(p: float):
+    """(forward, backward) scale of torch's dropout on the device: the fused kernel multiplies by fp32(1 / fp32(1 - p)),
+    its backward by fp32(1 / (1 - p)).  p == 1 drops everything (scale 0)."""
+    import numpy as np
+    if p >= 1.0:
+        return 0.0, 0.0
+    return float(np.float32(1.0 / float(np.float32(1.0 - p)))), float(np.float32(1.0 / (1.0 - p)))
+
+
+def _pgl_args(UA, IA, users, pos, neg, masks):
+    """Validated, contiguous operands of `mmrec_pgl_*` -- every check before anything reaches the device."""
+    if UA.dim() != 2 or IA.dim() != 2 or UA.shape[1] != IA.shape[1] or UA.shape[1] < 1:
+        raise MMRecError(f"pgl_loss: UA {tuple(UA.shape)} and IA {tuple(IA.shape)} must be [n_users, d] and [n_items, d]")
+    for name, t in (("users", users), ("pos", pos), ("neg", neg)):
+        if t.dim() != 1 or t.dtype not in (torch.int64, torch.int32):
+            raise MMRecError(f"pgl_loss: {name} must be a 1-D integer tensor")
+    B, d = users.numel(), UA.shape[1]
+    if B < 1 or pos.numel() != B or neg.numel() != B:
+        raise MMRecError(f"pgl_loss: users, pos and neg must hold the same B >= 1 entries, got {B}, {pos.numel()}, {neg.numel()}")
+    if masks is not None:
+        if len(masks) != 4:
+            raise MMRecError("pgl_loss: masks must be the four dropout masks of the views a, b, c, d, or None")
+        for m in masks:
+            if m.dtype not in (torch.bool, torch.uint8) or tuple(m.shape) != (B, d):
+                raise MMRecError(f"pgl_loss: every mask must be a bool [{B}, {d}] tensor, got {m.dtype} {tuple(m.shape)}")
+    _need_cuda(UA, IA, users, pos, neg, *(masks or ()))
+    idx = [t.to(torch.int64).contiguous() for t in (users, pos, neg)]
+    m = None if masks is None else [t.contiguous().view(torch.uint8) for t in masks]
+    return _f32c(UA), _f32c(IA), idx, m
+
+
+class _PglRowsFn(torch.autograd.Function):
+    """The row kernel: (x) or (x, a^, b^, c^, d^, pd); its backward takes K8's gradients of the views and the finish's of x and pd."""
+
+    @staticmethod
+    def forward(ctx, UA, IA, users, pos, neg, masks, p: float, want_cl: bool):
+        B, d = users.numel(), UA.shape[1]
+        dev = UA.device
+        scale, scale_bwd = dropout_scales(p) if masks is not None else (1.0, 1.0)
+        m = masks or [None] * 4
+        x = torch.empty(B, dtype=torch.float32, device=dev)
+        views = [torch.empty(B, d, dtype=torch.float32, device=dev) for _ in range(4)] if want_cl else [None] * 4
+        vnorm = torch.empty(4, B, dtype=torch.float32, device=dev) if want_cl else None
+        pd = torch.empty(2, B, dtype=torch.float32, device=dev) if want_cl else None
+        check(_lib.load().mmrec_pgl_rows_f32(B, d, _ptr(UA), _ptr(IA), _ptr(users), _ptr(pos), _ptr(neg), *map(_ptr, m), scale, _ptr(x),
+                                             *map(_ptr, views), _ptr(vnorm), _ptr(pd), _stream()), "mmrec_pgl_rows_f32")
+        ctx.save_for_backward(UA, IA, users, pos, neg, vnorm, *(masks or ()))
+        ctx.scales, ctx.want_cl, ctx.has_masks = (scale, scale_bwd), want_cl, masks is not None
+        return (x, *views, pd) if want_cl else x
+
+    @staticmethod
+    def backward(ctx, gx, *g_rest):
+        UA, IA, users, pos, neg, vnorm, *masks = ctx.saved_tensors
+        B, d = users.numel(), UA.shape[1]
+        m = masks if ctx.has_masks else [None] * 4
+        gv, gpd = ([_f32c(t) for t in g_rest[:4]], _f32c(g_rest[4])) if ctx.want_cl else ([None] * 4, None)
+        gU = torch.empty(B, d, dtype=torch.float32, device=UA.device)
+        gI = torch.empty(2 * B, d, dtype=torch.float32, device=UA.device)
+        scale, scale_bwd = ctx.scales
+        check(_lib.load().mmrec_pgl_rows_bwd_f32(B, d, _ptr(UA), _ptr(IA), _ptr(users), _ptr(pos), _ptr(neg), *map(_ptr, m), scale_bwd,
+                                                 scale, _ptr(_f32c(gx)), _ptr(vnorm), _ptr(gpd), *map(_ptr, gv), _ptr(gU), _ptr(gI),
+                                                 _stream()), "mmrec_pgl_rows_bwd_f32")
+        dU = index_sum_rows(gU, users, UA.shape[0]) if ctx.needs_input_grad[0] else None   # ascending j: bit-reproducible
+        dI = index_sum_rows(gI, torch.cat((pos, neg)), IA.shape[0]) if ctx.needs_input_grad[1] else None
+        return dU, dI, None, None, None, None, None, None
+
+
+class _PglFinishFn(torch.autograd.Function):
+    """The 0-dim loss from x and, with the InfoNCE terms, the positive dots and K8's two sums."""
+
+    @staticmethod
+    def forward(ctx, x, pd, ttl1, ttl2, reg_weight: float):
+        loss = torch.empty((), dtype=torch.float32, device=x.device)
+        check(_lib.load().mmrec_pgl_finish_f32(x.numel(), _ptr(x), _ptr(pd), _ptr(ttl1), _ptr(ttl2), reg_weight, _ptr(loss), _stream()),
+              "mmrec_pgl_finish_f32")
+        ctx.save_for_backward(x, pd, ttl1, ttl2)
+        ctx.reg_weight = reg_weight
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        x, pd, ttl1, ttl2 = ctx.saved_tensors
+        B = x.numel()
+        gx = torch.empty_like(x)
+        gpd = None if pd is None else torch.empty_like(pd)
+        gttl = None if pd is None else torch.empty(2, B, dtype=torch.float32, device=x.device)
+        check(_lib.load().mmrec_pgl_finish_bwd_f32(B, _ptr(x), _ptr(pd), _ptr(ttl1), _ptr(ttl2), ctx.reg_weight, _ptr(_f32c(g.reshape(1))),
+                                                   _ptr(gx), _ptr(gpd), _ptr(gttl), _stream()), "mmrec_pgl_finish_bwd_f32")
+        if pd is None:
+            return gx, None, None, None, None
+        return gx, gpd, gttl[0], gttl[1], None
+
+
+def pgl_loss(UA: torch.Tensor, IA: torch.Tensor, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor,
+             masks: Optional[Sequence[torch.Tensor]], dropout: float, reg_weight: float) -> torch.Tensor:
+    """PGL's `calculate_loss` after the tables (`src/models/pgl.py:227-259`): the 0-dim
+    `-mean(logsigmoid(<u, p> - <u, n>)) + reg_weight * (InfoNCE(a, b) + InfoNCE(c, d)) / 2` of the rows u = UA[users],
+    p = IA[pos], n = IA[neg], where a, b (c, d) are dropout draws of u (p) and InfoNCE has temperature 0.2.  `masks`: the
+    four bool [B, d] masks of the draws a, b, c, d (as `torch.native_dropout` returns them) for the dropout probability
+    `dropout`, or None when nothing is dropped (`nn.Dropout(0.0)`, or eval mode).  Differentiable w.r.t. UA and IA; the
+    table gradients are the per-row gradients scattered by `index_sum_rows`.
+
+    One row kernel each way (`mmrec_pgl_rows_f32` / `_bwd_f32`) and a one-CTA finish; the two B x B exp-sums are K8
+    (`expsum_rows`, forward and backward, so d must be 32, 64 or 128 unless reg_weight == 0).  reg_weight == 0 skips the
+    views, K8 and the InfoNCE arithmetic: `0 * cl` adds exact zeros while the inputs are finite.  Every element-wise step is
+    the torch expression's on the device; the batch sums are the same bits on every run.  Never synchronises with the host."""
+    UA, IA, (users, pos, neg), masks = _pgl_args(UA, IA, users, pos, neg, masks)
+    reg_weight = float(reg_weight)
+    want_cl = reg_weight != 0.0
+    if not want_cl:
+        x = _PglRowsFn.apply(UA, IA, users, pos, neg, masks, float(dropout), False)
+        return _PglFinishFn.apply(x, None, None, None, reg_weight)
+    if UA.shape[1] not in (32, 64, 128):
+        raise MMRecError(f"pgl_loss: the InfoNCE sums run on K8, which takes d = 32, 64 or 128, got {UA.shape[1]}")
+    x, a, b, c, d, pd = _PglRowsFn.apply(UA, IA, users, pos, neg, masks, float(dropout), True)
+    ttl1, ttl2 = expsum_rows(a, b, PGL_TAU), expsum_rows(c, d, PGL_TAU)
+    return _PglFinishFn.apply(x, pd, ttl1, ttl2, reg_weight)
 
 
 # ------------------------------------------------------------------------------------------------
